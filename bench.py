@@ -41,7 +41,10 @@ ALL_SECTIONS = ("parity", "weak", "gather", "tx90p", "bootstrap", "eqm", "batch5
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10,
+                    help="timed steps of the headline kernel (>= 1).  The secondary sections time min(steps, 5) "
+                         "(tx90p, e2e), min(steps, 3) (bootstrap, eqm, fwi) or min(steps, 2) (batch50, the e2e tx90p leg) "
+                         "calls, to bound the run at full size; each reports its own 'steps'")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--lat", type=int, default=Y_FULL, help="lat rows of the GLOBAL grid (default: full 721)")
@@ -51,7 +54,11 @@ def parse_args():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-tx90p", action="store_true")
     ap.add_argument("--cpu-lat", type=int, default=6, help="lat rows per worker of the bounded CPU sample")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs as DIR/<name>.npy (float32 / float64)")
     a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
     sec = [s for s in a.sections.split(",") if s]
     if a.no_e2e and "e2e" in sec:
         sec.remove("e2e")
@@ -210,6 +217,28 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------ our arm
+#: cells dumped over all ranks: 2 outputs x 30 periods x 4 B + an 8 B index = 248 B per cell, 32.5 MB in all
+DUMP_CELLS = 1 << 17
+
+
+def dump_outputs(path, out, valid, rank, world):
+    """The last timed step's outputs, (periods, cells) each, on a fixed seeded sample of DUMP_CELLS // world cells of
+    this rank's tile (all of them when the tile is smaller).  ``cells.npy`` holds the sampled cell indices within the
+    tile (float64, exact).  Under torchrun every rank writes its own tile with a ``.rank<r>`` suffix."""
+    import torch
+    os.makedirs(path, exist_ok=True)
+    C = out.shape[1]
+    n = DUMP_CELLS // world
+    cells = np.arange(C) if C <= n else np.sort(np.random.default_rng(0).choice(C, n, replace=False))
+    idx = torch.from_numpy(cells).to(out.device)
+    sfx = f".rank{rank}" if world > 1 else ""
+    arrays = {"max_consecutive_dry_days": out[:, idx].cpu().numpy().astype(np.float32),
+              "valid_count": valid[:, idx].cpu().numpy().astype(np.float32),
+              "cells": cells.astype(np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(path, f"{name}{sfx}.npy"), a)
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -283,6 +312,8 @@ def run_ours(args):
                 "kernel": "period_runstat_kernel<LT,MAX,VEC4,VALID,FASTMAX>",
                 "algorithmic_bytes": alg_bytes, "launch_ms": kern_ms, "tile": [T, ctx.rows, X],
                 "peak_source": ctx.peak["source"]}
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, out, valid, rank, world)
     out_max = float(out.max().item())
     n_missing = int((valid != YEAR).sum().item())
     assert 0 <= out_max <= YEAR
@@ -296,7 +327,7 @@ def run_ours(args):
                    "global_grid": [T, Yg, X],
                    "partition": f"one global grid, contiguous lat tiles over {world} rank(s): "
                                 + ",".join(str(b - a) for a, b in tiles) + " rows; no collective on the data path",
-                   "l2_policy": f"per-rank input {T * C * 4 / 1e9:.1f} GB >> 126 MB L2, read once per step "
+                   "l2_policy": f"per-rank input {T * C * 4 / 1e9:.1f} GB >> 50 MB L2, read once per step "
                                 "(no flush needed)"},
         "roofline": roofline, "gpu_launches": launches[0], "clocks": clk.summary(),
         "check": {"out_max_days": out_max, "periods_masked_missing": n_missing},

@@ -53,8 +53,8 @@ def main():
     import torch
     from xclim_b200 import _lib, device
     C = a.lat * X
-    peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", 6650.0) \
-        if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+    peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", 3350.0) \
+        if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0
     poff = np.arange(T // YEAR + 1, dtype=np.int32) * YEAR
     poff_m = None
     doy = (np.arange(T) % YEAR + 1).astype(np.int16)

@@ -1,5 +1,5 @@
 /*
- * xclim_b200 -- C ABI of the B200-native (sm_100a) per-grid-cell time-series kernels.
+ * xclim_b200 -- C ABI of the H100 (sm_90a) per-grid-cell time-series kernels.
  *
  * This is the drop-in boundary for ONE hot path of Ouranosinc/xclim (reference @ a8cbec8c):
  * the per-cell reductions behind `xclim.indices.run_length`, `xclim.indices.generic`,

@@ -100,9 +100,12 @@ def ffmc_step(t, p, w, h, f0):
 
 def dmc_step(t, p, h, mth, lat_band, d0):
     """Duff moisture code after one day (322-393).  ``lat_band`` = :func:`day_length_band` of the cells.
-    ``np.log(dmc0)`` is a float32 operation under numba (float32 argument), everything else float64."""
+    ``np.log(dmc0)`` is a float32 operation under numba (float32 argument), everything else float64.  numba
+    takes that logarithm from libm's logf, which nearly always equals the float64 log rounded once to float32;
+    numpy's vectorised float32 log is an ulp away from that for a few percent of arguments, so the rounded float64
+    log stands in for it, as it does in the device code."""
     with np.errstate(all="ignore"):
-        log_d0 = np.log(np.asarray(d0, dtype=np.float32)).astype(np.float64)
+        log_d0 = np.log(np.asarray(d0, dtype=np.float32).astype(np.float64)).astype(np.float32).astype(np.float64)
     t, p, h, d0 = (np.asarray(v, dtype=np.float64) for v in (t, p, h, d0))
     dl = DAY_LENGTHS[lat_band, int(mth) - 1]
     with np.errstate(all="ignore"):

@@ -1,11 +1,10 @@
 """Load the reference's pure numpy/numba cores WITHOUT copying them into this repo.
 
-The reference package cannot be imported in the authoring container (xarray, dask, pint ... are
-absent), but its numerical cores are plain numpy/numba functions.  This helper parses the
-reference source files where they lie (``/root/reference/src/xclim/...``), extracts the named
-top-level function definitions with ``ast`` and ``exec``s them in a private namespace.  It is used
-ONLY by ``make_golden.py`` (fixture generation, run in the authoring container) and by the
-``-m "not gpu"`` cross-check tests, which skip when ``/root/reference`` is absent (GPU box).
+The reference package need not be importable (xarray, dask, pint ... may be absent), but its numerical
+cores are plain numpy/numba functions.  This helper parses the reference source files where they lie
+(``$XCLIM_REFERENCE_ROOT/src/xclim/...``), extracts the named top-level function definitions with ``ast``
+and ``exec``s them in a private namespace.  It is used ONLY by ``make_golden.py``, which stores the
+reference's results as the ``tests/golden/*.npz`` fixtures; no test reads the reference sources.
 """
 from __future__ import annotations
 
@@ -17,7 +16,7 @@ from collections.abc import Sequence
 
 import numpy as np
 
-REF_ROOT = os.environ.get("XCLIM_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("XCLIM_REFERENCE_ROOT", "")
 
 RUN_LENGTH_FUNCS = [
     "_cumsum_reset_np", "_rle_1d", "rle_1d", "first_run_1d", "statistics_run_1d",

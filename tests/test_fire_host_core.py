@@ -6,7 +6,7 @@ import pytest
 
 import fwi_host_build as hb
 from oracle import fire_oracle as FO
-from test_fire_oracle import case_inputs, check_outputs, golden, mg  # noqa: F401
+from test_fire_oracle import case_inputs, check_outputs, cross, golden, mg  # noqa: F401
 
 
 @pytest.mark.parametrize("name", list(mg.CFFWIS_CASES))
@@ -90,59 +90,54 @@ def test_elementwise_functions_of_the_host_build(golden):  # noqa: F811
     assert hb.elementwise("BUI", np.zeros(1, np.float32), np.zeros(1, np.float32))[0] == 0
 
 
-@pytest.mark.skipif(not __import__("_ref_extract").available(), reason="reference sources not present (GPU box)")
-def test_every_mode_combination_against_the_live_reference():
+def on_stored_days(got, outs, case):
+    """Outputs ``outs`` of ``got``, in that order, cut to the days the fixture stores for case number ``case``."""
+    return {o: (np.asarray(got[o])[case % mg.DAY_STRIDE::mg.DAY_STRIDE] if np.asarray(got[o]).ndim == 2 else
+                np.asarray(got[o])) for o in outs}
+
+
+class StoredReference:
+    """Reads back the reference's outputs of one cross-check family in the order tests/golden/make_golden.py stored
+    them (cross_check_fixture): case by case, output by output, the stored days of each."""
+
+    def __init__(self, cross, tag):
+        self.streams = {False: cross[f"{tag}/values"], True: cross[f"{tag}/masks"]}
+        self.pos = {False: 0, True: 0}
+
+    def take(self, like):
+        """The reference's values for the next case, shaped as ``like`` (output -> (days, C) or (C,) array)."""
+        exp = {}
+        for o, a in like.items():
+            m = o == "season_mask"
+            p = self.pos[m]
+            block = self.streams[m][p:p + a.size]
+            assert block.size == a.size, f"{o}: the stored stream ends early"
+            exp[o] = block.reshape(a.shape[::-1]).T if a.ndim == 2 else block
+            self.pos[m] = p + a.size
+        return exp
+
+    def assert_consumed(self):
+        assert all(self.pos[m] == self.streams[m].size for m in self.pos), "stored values left over"
+
+
+def test_every_mode_combination_against_the_reference(cross):  # noqa: F811
     """All combinations of season method x overwintering x dry start x initial_start_up, each with random
     thresholds / window lengths / previous codes: the oracle AND the host build of the device code against the
-    reference's `_fire_weather_calc` executed where it lies."""
-    import itertools
-    import warnings
-
-    import _ref_extract as ref
-    fw = ref.load_cffwis()
-    rng = np.random.default_rng(123)
-    T = 320
-    combos = itertools.product([None, "mask", "WF93", "LA08", "GFWED"], [False, True], [None, "CFS", "GFWED", "GFWED+SNOW"],
-                               [True, False])
+    reference's `_fire_weather_calc` on the same inputs (stored results)."""
     n = 0
-    for trial, (season, ow, dry, isu) in enumerate(combos):
-        if ow and season is None:
-            continue
-        inp = mg.cffwis_inputs(seed=1000 + trial, C=16, T=T)
-        dc0, dmc0, ffmc0, wpr = mg.cffwis_state(inp, [None, "some", "all"][trial % 3])
-        over = dict(season_method=season, overwintering=ow, dry_start=dry, initial_start_up=isu,
-                    temp_condition_days=int(rng.integers(1, 6)), snow_condition_days=int(rng.integers(1, 6)),
-                    snow_cover_days=int(rng.integers(5, 70)), temp_start_thresh=float(rng.uniform(8, 14)),
-                    temp_end_thresh=float(rng.uniform(2, 7)), snow_thresh=float(rng.choice([0.01, 0.03])),
-                    prec_thresh=float(rng.choice([1.0, 2.5])), dc_dry_factor=int(rng.integers(2, 7)),
-                    dmc_dry_factor=int(rng.integers(1, 4)), snow_min_cover_frac=float(rng.uniform(0.3, 0.8)),
-                    snow_min_mean_depth=float(rng.uniform(0.02, 0.1)), carry_over_fraction=float(rng.choice([0.5, 0.75, 1.0])),
-                    wetting_efficiency_fraction=float(rng.choice([0.5, 0.75, 0.9])))
-        outs = ["DC", "DMC", "FFMC", "ISI", "BUI", "FWI", "DSR"]
-        mask = None
-        if season == "mask":                      # a persistent random mask
-            mask = np.zeros((16, T), bool)
-            st = rng.random(16) < 0.5
-            for t in range(T):
-                st = np.where(rng.random(16) < 0.03, ~st, st)
-                mask[:, t] = st
-        elif season is not None:
-            outs.append("season_mask")
-        if ow:
-            outs.append("winter_pr")
-        kw = mg.cffwis_params(fw, outputs=outs, **over)
-        with warnings.catch_warnings():
-            warnings.simplefilter("ignore")
-            res = fw["_fire_weather_calc"](inp["tas"], inp["pr"], inp["hurs"], inp["ws"], inp["snd"], inp["mth"], inp["lat"],
-                                           mask, dc0.copy(), dmc0.copy(), ffmc0.copy(), wpr.copy(), **kw)
-        exp = {o: (np.asarray(a).T if np.asarray(a).ndim == 2 else np.asarray(a)) for o, a in zip(outs, res)}
+    ref = StoredReference(cross, "modes")
+    for i, (inp, mask, (dc0, dmc0, ffmc0, wpr), over, outs) in enumerate(mg.mode_combinations()):
         tc = lambda a: np.ascontiguousarray(a.T)   # noqa: E731
         args = (tc(inp["tas"]), tc(inp["pr"]), tc(inp["hurs"]), tc(inp["ws"]), tc(inp["snd"]), inp["mth"], inp["lat"],
                 None if mask is None else np.ascontiguousarray(mask.T), dc0, dmc0, ffmc0, wpr)
-        label = f"{season},{ow},{dry},{isu}"
-        check_outputs(FO.fire_weather_calc(*args, outputs=outs, **over), exp, "oracle:" + label, exact_frac=0.98)
-        check_outputs(hb.run(*args, outputs=outs, **over), exp, "host build:" + label, exact_frac=0.98)
+        label = f"{over['season_method']},{over['overwintering']},{over['dry_start']},{over['initial_start_up']}"
+        oracle = on_stored_days(FO.fire_weather_calc(*args, outputs=outs, **over), outs, i)
+        exp = ref.take(oracle)
+        check_outputs(oracle, exp, "oracle:" + label, exact_frac=0.98)
+        check_outputs(on_stored_days(hb.run(*args, outputs=outs, **over), outs, i), exp, "host build:" + label,
+                      exact_frac=0.98)
         n += 1
+    ref.assert_consumed()
     assert n == 72
 
 
@@ -163,43 +158,21 @@ def test_ring_mean_rounds_as_numpy_mean():
             assert np.float32(got) == np.mean(vals), (n, head)
 
 
-@pytest.mark.skipif(not __import__("_ref_extract").available(), reason="reference sources not present (GPU box)")
-def test_branch_point_inputs_against_the_live_reference():
-    """Inputs drawn from the branch points of the equations (rain thresholds 0.5 / 1.5 / 2.8 mm and just above,
-    humidity 0 and 100 %, calm and storm winds, temperatures at -2.8 / -1.1 / 21.1 degC, snow depth at its
-    threshold, latitudes on the band edges, previous codes at 0 / 33 / 65 / 101), with and without missing
-    values: oracle and host build of the device code against the reference executed where it lies."""
-    import warnings
-
-    import _ref_extract as ref
-    fw = ref.load_cffwis()
-    rng = np.random.default_rng(7)
-    C, T = 32, 240
-    f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)   # noqa: E731
-    for trial in range(6):
-        tas = rng.choice([-45.0, -2.8, -1.1, 0.0, 21.1, 35.0, 50.0], size=(C, T)) + rng.normal(0, 0.5, (C, T))
-        pr = rng.choice([0.0, 0.5, 0.50001, 1.5, 1.50001, 2.8, 2.80001, 50.0, 300.0], size=(C, T))
-        hurs = rng.choice([0.0, 1e-3, 5.0, 50.0, 99.999, 100.0], size=(C, T))
-        ws = rng.choice([0.0, 1e-3, 10.0, 100.0, 250.0], size=(C, T))
-        snd = rng.choice([0.0, 0.01, 0.010001, 0.5], size=(C, T))
-        if trial % 3 == 0:
-            for a in (tas, pr, hurs, ws):
-                a[rng.random((C, T)) < 0.002] = np.nan
-        mth = rng.integers(1, 13, T).astype(np.int64)
-        lat = rng.choice([-90, -30, -15, 15, 30, 90, -29.999, 14.999, 0], size=C).astype(np.float64)
-        dc0, dmc0, ffmc0, wpr = mg.cffwis_state({"tas": f32(tas)}, [None, "some", "all"][trial % 3])
-        if trial % 3:
-            dc0[:4], dmc0[:4], ffmc0[:4] = [0.0, 1e-3, 800.0, 2000.0], [0.0, 33.0, 65.0, 500.0], [0.0, 101.0, 50.0, 99.9]
-        for season, ow, dry in ((None, False, None), ("WF93", True, "CFS"), ("GFWED", False, "GFWED+SNOW"), ("LA08", True, None)):
-            outs = ["DC", "DMC", "FFMC", "ISI", "BUI", "FWI", "DSR"] + (["season_mask"] if season else []) + \
-                (["winter_pr"] if ow else [])
-            over = dict(season_method=season, overwintering=ow, dry_start=dry, snow_cover_days=10)
-            kw = mg.cffwis_params(fw, outputs=outs, **over)
-            with warnings.catch_warnings():
-                warnings.simplefilter("ignore")
-                res = fw["_fire_weather_calc"](f32(tas), f32(pr), f32(hurs), f32(ws), f32(snd), mth, lat, None, dc0.copy(),
-                                               dmc0.copy(), ffmc0.copy(), wpr.copy(), **kw)
-            exp = {o: (np.asarray(a).T if np.asarray(a).ndim == 2 else np.asarray(a)) for o, a in zip(outs, res)}
-            args = tuple(f32(a.T) for a in (tas, pr, hurs, ws, snd)) + (mth, lat, None, dc0, dmc0, ffmc0, wpr)
-            check_outputs(FO.fire_weather_calc(*args, outputs=outs, **over), exp, f"oracle {trial} {season}", exact_frac=0.97)
-            check_outputs(hb.run(*args, outputs=outs, **over), exp, f"host build {trial} {season}", exact_frac=0.97)
+def test_branch_point_inputs_against_the_reference(cross):  # noqa: F811
+    """Inputs drawn from the branch points of the equations (tests/golden/make_golden.py: branch_point_cases), with
+    and without missing values: oracle and host build of the device code against the reference's results on the
+    same inputs (stored results)."""
+    n = 0
+    ref = StoredReference(cross, "branch")
+    for i, (inp, (dc0, dmc0, ffmc0, wpr), over, outs) in enumerate(mg.branch_point_cases()):
+        args = tuple(np.ascontiguousarray(inp[k].T) for k in ("tas", "pr", "hurs", "ws", "snd")) + \
+            (inp["mth"], inp["lat"], None, dc0, dmc0, ffmc0, wpr)
+        label = f"{i} {over['season_method']}"
+        oracle = on_stored_days(FO.fire_weather_calc(*args, outputs=outs, **over), outs, i)
+        exp = ref.take(oracle)
+        check_outputs(oracle, exp, f"oracle {label}", exact_frac=0.97)
+        check_outputs(on_stored_days(hb.run(*args, outputs=outs, **over), outs, i), exp, f"host build {label}",
+                      exact_frac=0.97)
+        n += 1
+    ref.assert_consumed()
+    assert n == 24

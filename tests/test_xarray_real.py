@@ -45,7 +45,7 @@ def test_dataarrays_in_dataarrays_out(cuda):
 
 
 def test_registered_under_the_xclim_indicator_registry(cuda):
-    """INTEGRATION.md route (a): bind the B200 index as ``compute`` of a stock indicator and compare with
+    """INTEGRATION.md route (a): bind the xclim_b200 index as ``compute`` of a stock indicator and compare with
     stock xclim on the same input (engages only where xclim imports)."""
     xclim = pytest.importorskip("xclim")
     from xclim.core.indicator import Indicator

@@ -1,5 +1,4 @@
-"""GPU tests of host-layer compositions added after the GPU budget of round 2 was spent (existing, verified
-kernels in new combinations); not yet run on hardware, hence the file name that sorts late."""
+"""GPU tests of host-layer compositions: existing, verified kernels in new combinations."""
 import numpy as np
 import pytest
 

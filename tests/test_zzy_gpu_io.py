@@ -1,6 +1,5 @@
-"""GPU: file-backed lazy sources (NetCDF-3, zarr v2) through the slab streamer (SURVEY.md 8f.3).
-Added after the GPU budget of round 2 was spent: the host logic runs in tests/test_io_formats.py on CPU
-stand-ins; these have not run on hardware yet (hence the file name that sorts last)."""
+"""GPU: file-backed lazy sources (NetCDF-3, zarr v2) through the slab streamer (SURVEY.md 8f.3).  The host logic
+also runs in tests/test_io_formats.py on CPU stand-ins."""
 import numpy as np
 import pytest
 

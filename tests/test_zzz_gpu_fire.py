@@ -1,9 +1,8 @@
 """GPU: the fire-weather kernel (xc_fwi_f32) through the C ABI against the reference fixtures, the oracle and
-through the host layer.  Written after the GPU budget of round 2 was spent: these have NOT run on hardware
-yet (hence the file name that sorts last, and the looser share of bit-identical values asked for: CUDA's logf /
-exp / pow differ from glibc's by an ulp now and then, which flips a float32 rounding that the recurrences then
-carry for days; every value must still agree to 2e-6); the kernel's device code is verified on the CPU as a host build
-(tests/test_fire_host_core.py)."""
+through the host layer.  A looser share of bit-identical values is asked for than on the CPU: CUDA's float64 exp /
+log / pow differ from glibc's by an ulp now and then, which flips a float32 rounding that the recurrences then
+carry for days; every value must still agree to 2e-6.  The kernel's device code is also verified on the CPU as a
+host build (tests/test_fire_host_core.py)."""
 import numpy as np
 import pytest
 
@@ -96,7 +95,7 @@ def test_fire_weather_streams_from_files_on_device(cuda, tmp_path):
 
 def test_kernel_every_mode_combination_against_the_oracle(cuda):
     """All season x overwintering x dry-start x initial_start_up combinations with random parameters: the kernel
-    against the oracle, which tests/test_fire_host_core.py pins to the live reference on the SAME combinations
+    against the oracle, which tests/test_fire_host_core.py pins to the reference on the SAME combinations
     (there, with the host build of this kernel's device code)."""
     import itertools
     rng = np.random.default_rng(123)
@@ -140,7 +139,7 @@ def test_kernel_every_mode_combination_against_the_oracle(cuda):
 
 
 def test_kernel_branch_point_inputs_against_the_oracle(cuda):
-    """The branch-point inputs of tests/test_fire_host_core.py::test_branch_point_inputs_against_the_live_reference
+    """The branch-point inputs of tests/test_fire_host_core.py::test_branch_point_inputs_against_the_reference
     (there: oracle and host build against the reference), here the kernel against the oracle."""
     rng = np.random.default_rng(7)
     C, T = 32, 240

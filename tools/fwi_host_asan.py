@@ -1,18 +1,22 @@
 """The host build of the fire-weather device code under AddressSanitizer + UBSan (every fixture case and the
-longest rings).  Run:
+longest rings).  Run from the repository root:
 
     g++ -O1 -g -std=c++17 -ffp-contract=off -fPIC -shared -fsanitize=address,undefined -fno-omit-frame-pointer \\
-        -I/usr/local/cuda/include tests/csrc/fwi_host.cpp -o /tmp/libfwi_asan.so
-    LD_PRELOAD=$(g++ -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 python tools/fwi_host_asan.py
+        -I/usr/local/cuda/include tests/csrc/fwi_host.cpp -o build/libfwi_asan.so
+    LD_PRELOAD=$(g++ -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 python tools/fwi_host_asan.py build/libfwi_asan.so
 """
 import sys, os, ctypes
-sys.path.insert(0,'/root/repo/tests'); sys.path.insert(0,'/root/repo'); sys.path.insert(0,'/root/repo/tests/golden')
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for d in (os.path.join(ROOT, "tests"), ROOT, os.path.join(ROOT, "tests", "golden")):
+    sys.path.insert(0, d)
+if len(sys.argv) != 2:
+    raise SystemExit(__doc__)
 import numpy as np
 import fwi_host_build as hb
-hb._lib = ctypes.CDLL('/tmp/libfwi_asan.so'); hb._lib.fwi_host_last_error.restype = ctypes.c_char_p
+hb._lib = ctypes.CDLL(os.path.abspath(sys.argv[1])); hb._lib.fwi_host_last_error.restype = ctypes.c_char_p
 import make_golden as mg
 from test_fire_oracle import case_inputs, check_outputs
-g = np.load('/root/repo/tests/golden/ref_cffwis.npz')
+g = np.load(os.path.join(ROOT, "tests", "golden", "ref_cffwis.npz"))
 for name in mg.CFFWIS_CASES:
     args, kw, exp = case_inputs(g, name)
     got = hb.run(*args, **kw)

@@ -1,4 +1,4 @@
-"""xclim_b200 -- B200-native (sm_100a) kernels behind xclim's per-grid-cell time-series API.
+"""xclim_b200 -- H100 (sm_90a) CUDA kernels behind xclim's per-grid-cell time-series API.
 
 Only the hot path named by BASELINE.json is implemented (SURVEY.md section 8); units, metadata,
 checks and the Indicator machinery stay with the reference.  Importing this package does not load

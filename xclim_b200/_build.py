@@ -1,4 +1,4 @@
-"""Build ``libxclim_b200.so`` in-tree with nvcc for sm_100a (no torch, no cmake).
+"""Build ``libxclim_b200.so`` in-tree with nvcc for sm_90a (H100; no torch, no cmake).
 
 ``python -m xclim_b200._build`` (or ``__graft_entry__.build()``) compiles every ``csrc/*.cu`` to an
 object under ``build/`` and links ``xclim_b200/lib/libxclim_b200.so``.  nvcc cross-compiles without
@@ -19,8 +19,11 @@ LIB_DIR = os.path.join(PKG, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libxclim_b200.so")
 OBJ_DIR = os.path.join(ROOT, "build", "obj")
 
+#: the one target architecture: Hopper (H100, sm_90a)
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
+
 NVCC_FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", *ARCH_FLAGS, "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "--extended-lambda",
     "-Xptxas", "-v", "-Wno-deprecated-gpu-targets",
 ]
@@ -63,7 +66,7 @@ def build_variant(tag: str, defines: list[str]) -> str:
         if r.returncode != 0:
             raise RuntimeError(r.stderr)
         objs.append(obj)
-    r = subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", out, *objs],
+    r = subprocess.run([nvcc, "-shared", *ARCH_FLAGS, "-o", out, *objs],
                        capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(r.stderr)
@@ -107,7 +110,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     need_link = force or bool(jobs) or not os.path.exists(LIB_PATH) or any(
         os.path.getmtime(o) > os.path.getmtime(LIB_PATH) for o in objs)
     if need_link:
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH, *objs]
+        cmd = [nvcc, "-shared", *ARCH_FLAGS, "-o", LIB_PATH, *objs]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

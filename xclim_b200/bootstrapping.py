@@ -1,4 +1,4 @@
-"""B200 implementation behind ``xclim.core.bootstrapping`` (percentile bootstrap, Zhang 2005)."""
+"""CUDA implementation behind ``xclim.core.bootstrapping`` (percentile bootstrap, Zhang 2005)."""
 from __future__ import annotations
 
 import numpy as np

@@ -1,4 +1,4 @@
-"""B200 implementations behind ``xclim.core.calendar.percentile_doy`` / ``resample_doy``."""
+"""CUDA implementations behind ``xclim.core.calendar.percentile_doy`` / ``resample_doy``."""
 from __future__ import annotations
 
 import weakref

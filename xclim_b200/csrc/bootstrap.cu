@@ -604,7 +604,7 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
 int32_t launch_bootstrap5(int32_t op, const float* x, int64_t C, int64_t ldx, int64_t base_start, int32_t N, int32_t L,
                           const QuantSpec& spec, const int32_t* step_period, int32_t* counts, cudaStream_t st) {
   const int64_t cblocks = (C + kBT - 1) / kBT;
-  int chunks = (int)((148 * 12 + cblocks - 1) / cblocks);
+  int chunks = (int)((sm_count() * 12 + cblocks - 1) / cblocks);
   chunks = chunks < 1 ? 1 : chunks;
   int per = (L + chunks - 1) / chunks;
   if (per < 20) per = 20;
@@ -635,7 +635,7 @@ int32_t launch_bootstrap(int32_t op, const float* x, int64_t C, int64_t ldx, int
                          int32_t L, int32_t W, const QuantSpec& spec, const int32_t* step_period, int32_t* counts,
                          cudaStream_t st) {
   const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  int chunks = (int)((148 * 6 + cblocks - 1) / cblocks);
+  int chunks = (int)((sm_count() * 6 + cblocks - 1) / cblocks);
   chunks = chunks < 1 ? 1 : chunks;
   int per = (L + chunks - 1) / chunks;
   if (per < 4 * W) per = 4 * W;

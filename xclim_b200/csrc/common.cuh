@@ -1,4 +1,4 @@
-// Shared helpers for the xclim_b200 kernels (sm_100a only).
+// Shared helpers for the xclim_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -99,5 +99,16 @@ inline int32_t dispatch_op_nan(int32_t op, F&& f) {
 }
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// SMs of the current device (132 on an H100 SXM, 114 on an H100 PCIe): launchers that split a narrow grid
+// into more CTAs size the split by it.  The split never changes a result, only how the work is spread.
+inline int sm_count() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return 132;
+  }
+  return n;
+}
 
 }  // namespace xc

@@ -8,7 +8,7 @@
 //   adjust: scen = sim (+|*) interp(sim; hist_q -> af), nearest or linear, constant extrapolation.
 // Reference call sites: tests/test_xsdba.py:21-34, 143-150.
 //
-// Design (B200).  train needs ~2*nq order statistics spread over the WHOLE distribution of a
+// Design.  train needs ~2*nq order statistics spread over the WHOLE distribution of a
 // 10950-sample series, i.e. a real per-cell sort: one CTA owns one cell, gathers its series into
 // shared memory (64 KB for 16384 keys) and runs a bitonic sort there; neighbouring cells are
 // handled by neighbouring CTAs at the same time so that the 32-byte sectors fetched by the strided
@@ -260,12 +260,12 @@ eqm_train_kernel(const float* __restrict__ ref, const float* __restrict__ hist, 
 // train, a GROUP of adjacent cells per CTA: the same multi-select (min/max -> 1024-bin histogram -> gather the
 // wanted bins -> rank by counting), but a CTA owns kG adjacent cells, i.e. kG * 4 contiguous bytes of every
 // time row, and every fetched sector is used whole (the one-cell kernel fetched each sector for eight CTAs:
-// ncu r1 capture E, 4 useful bytes per 32-byte sector).
+// 4 useful bytes per 32-byte sector).
 //
-// What bounds it (measured, r2): the number of (CTA, time row) TOUCHES.  At a 4 MB row stride every row of a
-// CTA's slice lies in another DRAM page, and both earlier variants ran at the same ~28 G touches/s whatever the
-// bytes per touch (16 cells x 3 sweeps: 4.3 G touches in 150 ms; 4 cells staged in shared memory x 1 sweep:
-// 5.7 G touches in 203 ms).  So the group is as WIDE as shared memory allows -- 32 cells = 128 bytes per touch --
+// What bounds it: the number of (CTA, time row) TOUCHES.  At a 4 MB row stride every row of a CTA's slice
+// lies in another DRAM page, and both earlier variants ran at the same rate of touches whatever the bytes per
+// touch (16 cells x 3 sweeps: 4.3 G touches; 4 cells staged in shared memory x 1 sweep: 5.7 G touches, and
+// slower by that ratio).  So the group is as WIDE as shared memory allows -- 32 cells = 128 bytes per touch --
 // which needs the per-cell state small:
 //   * the packed histogram (two 16-bit counters per word, T <= 32768) and the candidate pool share one
 //     1024-word block per cell (the prefix sums are dead once the candidate offsets are known);
@@ -622,8 +622,8 @@ constexpr int kAdjThreads = 128;
 constexpr int kLut = 32;   // coarse position table per cell
 
 // adjust: a lane owns a cell and streams its series.  Per element the segment of the quantile table is found
-// through a 32-entry position table of the cell instead of a 5-step bisection (ncu r1: ~45 instructions per
-// element, issue-bound at 0.36 of the HBM roofline): b = bin(x) on a uniform grid over [hq[0], hq[nq-1]],
+// through a 32-entry position table of the cell instead of a 5-step bisection (~45 instructions per element,
+// issue-bound): b = bin(x) on a uniform grid over [hq[0], hq[nq-1]],
 // lut[b] = #{ j : bin(hq[j]) < b } is a LOWER bound of idx = #{ hq[j] < x } (bin() is monotone, so a node in a
 // lower bin is below x), and the few nodes sharing x's bin are settled by a short forward scan -- two
 // unconditional steps, then a loop that almost never runs.  Same idx, same arithmetic, bit-identical output.
@@ -774,7 +774,7 @@ extern "C" int32_t xc_eqm_train_f32(const float* ref, const float* hist, int64_t
   const int64_t need = xc_eqm_train_workspace_bytes(T, C, nq);
   // widest group first: 32 cells = 128 bytes per (CTA, time row) touch; 16 when C is not a multiple of 32 or the
   // targets of 32 cells do not fit in shared memory.  (A variant that staged a 4-cell slice in shared memory and
-  // read DRAM once was a measured NEGATIVE result -- 203 ms vs 150 ms: four times the row touches -- and is gone.)
+  // read DRAM once was slower -- four times the row touches -- and is gone.)
   const char* kg_env = getenv("XCLIM_B200_EQM_KG");
   const char* gt_env = getenv("XCLIM_B200_EQM_GT");
   int g = 32;
@@ -805,7 +805,7 @@ extern "C" int32_t xc_eqm_train_f32(const float* ref, const float* hist, int64_t
   int32_t e = launch_status("eqm_train_group_kernel");
   if (e) return e;
   // cells the eight-cell layout could not finish (heavy non-constant bins): a small fixed grid walks the list
-  return launch_train_cells(ref, hist, T, C, ldx, nq, kind, af, hist_q, redo, 296u, st);
+  return launch_train_cells(ref, hist, T, C, ldx, nq, kind, af, hist_q, redo, 2u * (unsigned)sm_count(), st);
 }
 
 extern "C" int32_t xc_eqm_adjust_f32(const float* sim, int64_t T, int64_t C, int64_t ldx, const float* af,
@@ -818,7 +818,7 @@ extern "C" int32_t xc_eqm_adjust_f32(const float* sim, int64_t T, int64_t C, int
   XC_REQUIRE(interp == 0 || interp == 1, "interp must be 0 (nearest) or 1 (linear)");
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t cblocks = (C + kAdjThreads - 1) / kAdjThreads;
-  int tchunks = (int)((148 * 16 + cblocks - 1) / cblocks);
+  int tchunks = (int)((sm_count() * 16 + cblocks - 1) / cblocks);
   tchunks = tchunks < 1 ? 1 : tchunks;
   int rows = (int)((T + tchunks - 1) / tchunks);
   if (rows < 64) rows = 64;

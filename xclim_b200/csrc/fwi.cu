@@ -75,7 +75,8 @@ extern "C" int32_t xc_fwi_elementwise_f32(int32_t kind, const float* a, const fl
   XC_REQUIRE(a && out && (b || kind == XC_FWI_EW_DSR), "null pointer argument");
   XC_REQUIRE(n > 0, "bad shape");
   const int64_t want = (n + 255) / 256;
-  const unsigned blocks = (unsigned)(want < 148 * 16 ? want : 148 * 16);   // grid-stride: 16 CTAs per SM at most
+  const int64_t cap = (int64_t)sm_count() * 16;   // grid-stride: 16 CTAs per SM at most
+  const unsigned blocks = (unsigned)(want < cap ? want : cap);
   fwi_elementwise_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(kind, a, b, n, p0, p1, p2, out);
   return launch_status("fwi_elementwise_kernel");
 }

@@ -97,6 +97,12 @@ XC_FWI_HD double ffmc_step(float t_, float p_, float w_, float h_, float f0_) {
   return ffmc;
 }
 
+// np.log of a float32 argument inside the reference's numba code: libm's logf, within an ulp of the exact value
+// and nearly always equal to the float64 log rounded once to float32 (glibc: all but about 1 argument in 2,000).
+// CUDA's logf and numpy's vectorised float32 log differ from it far more often, and an ulp in Eq. 13 is magnified
+// about fifty-fold where Eq. 15 cancels to a small DMC after rain, so host and device both round the float64 log.
+XC_FWI_HD float log_f32(float x) { return (float)log((double)x); }
+
 // _duff_moisture_code (:322-393); dl = day length of the cell's band for the month.
 XC_FWI_HD double dmc_step(float t_, float p_, float h_, double dl, float d0_) {
   if (d0_ != d0_) return (double)NAN;
@@ -108,8 +114,8 @@ XC_FWI_HD double dmc_step(float t_, float p_, float h_, double dl, float d0_) {
     const double wmi = 20.0 + 280.0 / exp(0.023 * d0);                                // Eq. 12 (cffdrs)
     double b;
     if (d0 <= 33.0) b = 100.0 / (0.5 + 0.3 * d0);                                     // Eq. 13a
-    else if (d0 <= 65.0) b = 14.0 - 1.3 * (double)logf(d0_);                          // Eq. 13b
-    else b = 6.2 * (double)logf(d0_) - 17.2;                                          // Eq. 13c
+    else if (d0 <= 65.0) b = 14.0 - 1.3 * (double)log_f32(d0_);                       // Eq. 13b
+    else b = 6.2 * (double)log_f32(d0_) - 17.2;                                       // Eq. 13c
     const double wmr = wmi + (1000.0 * rw) / (48.77 + b * rw);                        // Eq. 14
     pr = 43.43 * (5.6348 - log(wmr - 20.0));                                          // Eq. 15 (cffdrs)
   } else {

@@ -6,7 +6,7 @@
 //
 // Sample of day-of-year d (window w = 2h+1):  S(d) = { x[i+k] : doy(i) = d, |k| <= h, 0 <= i+k < T }.
 //
-// Design (B200).  The (time, lat, lon) buffer is coalesced along cells, so a LANE owns one cell
+// Design.  The (time, lat, lon) buffer is coalesced along cells, so a LANE owns one cell
 // (a warp reads one 128-byte row segment per time step) and keeps the order statistics it needs in
 // REGISTERS: only the K extreme values of S(d) matter (K = 16 for the 90th percentile of 150
 // samples), never the full sort the reference does.
@@ -182,7 +182,7 @@ percentile_doy_select_kernel(const float* __restrict__ x, int64_t T, int64_t C, 
 #define XC_PCTL_ADDR (XC_PCTL_VARIANT == 1 ? 1 : 0)
 #endif
 #ifndef XC_PCTL_STAGE     // 1: cp.async staging of the next day's rows in the window-5 paired kernel
-#define XC_PCTL_STAGE 1      // (an L2 prefetch of those rows was measured SLOWER: 16.1 vs 13.7 ms)
+#define XC_PCTL_STAGE 1      // (an L2 prefetch of those rows was slower)
 #endif
 #ifndef XC_PCTL_PROBE     // NaN probe: 0 = compare chain (ALU pipe); 1 = FMA chain; 2 = FADD tree + 1 compare per 4
 #define XC_PCTL_PROBE (XC_PCTL_VARIANT == 1 ? 1 : 0)
@@ -261,7 +261,7 @@ __device__ __forceinline__ void load_sort_chunk(const char* p0, uint64_t ystride
 
 // ---- asynchronous staging of the NEXT day's rows (cp.async, global -> shared) --------------------
 // The day-list kernels are bound by the min/max pipe but lose a third of their issue slots waiting
-// for the 30 row loads of a day (ncu: long_scoreboard 35 %).  With a Stager the rows of day e+1 are
+// for the 30 row loads of a day (long-scoreboard stalls).  With a Stager the rows of day e+1 are
 // copied to a per-lane shared-memory column while day e is sorted and merged; a lane reads back only
 // what it copied itself, so cp.async.wait_group is the only synchronisation.  The buffer is reused
 // chunk by chunk: as soon as the 16 (14) values of a chunk are in registers, the copy of the same
@@ -496,11 +496,11 @@ __device__ __forceinline__ float fold_thr(double t) {
 }
 
 
-#ifndef XC_PCTL_PAIR_MINBLOCKS   // with the staging buffer 4 CTAs fit an SM (51 KB each): 13.33 ms;
-#define XC_PCTL_PAIR_MINBLOCKS 4  // 6 (80 registers) gives 13.59 ms, no staging 13.65 ms
+#ifndef XC_PCTL_PAIR_MINBLOCKS   // with the staging buffer 4 CTAs fit an SM (51 KB each)
+#define XC_PCTL_PAIR_MINBLOCKS 4
 #endif
-// (The day-by-day window-5 kernel with the fused per-year count of the same series -- tx90p sub-case 3a in one
-// pass -- was removed in round 2: 38 ms against 10.5 + 7.1 ms for the two-kernel path.)
+// (A day-by-day window-5 kernel with the fused per-year count of the same series -- tx90p sub-case 3a in one
+// pass -- was slower than the two-kernel path and was removed.)
 // Window 5, days handled in PAIRS.  With B(d) = Y(d-2..d+1) = A(d-1) U A(d+1) the windows of two
 // neighbouring days are one rank-only merge away:  S(d-1) = Y(d-3) U B(d)  and  S(d) = B(d) U Y(d+2).
 // Per pair of days: one pair merge A(d+1), one merge B(d), two rank-only finals (2*80 + 2*32
@@ -508,7 +508,7 @@ __device__ __forceinline__ float fold_thr(double t) {
 // values of a day (the larger part of the work) is unchanged.
 // The loop still advances ONE day per iteration (even/odd branch) so that the body holds a single
 // copy of the day-list sort and of the final merge: two inlined copies overflow the 32 KB
-// instruction cache and cost more than the saved merges (measured: 17.1 ms vs 15.5 ms).
+// instruction cache and cost more than the saved merges.
 // Shared memory per lane: A(d-1), the two most recent odd-position day lists Y(d-3), Y(d-1), and
 // the even-position list Y(d) waiting for its partner.
 template <int K, bool TABLE>
@@ -612,12 +612,11 @@ percentile_doy_w5p_kernel(const float* __restrict__ x, int32_t T, int64_t C, int
 
 
 // ------------------------------------------------------------------------------------------------
-// Window 5, paired days, rows delivered by TMA (sm_100a: cp.async.bulk.tensor + mbarrier).
+// Window 5, paired days, rows delivered by TMA (sm_90a: cp.async.bulk.tensor + mbarrier).
 //
 // Same arithmetic as percentile_doy_w5p_kernel (identical networks, identical results), but the N
 // rows of a day-of-year are no longer fetched lane by lane (N loads, 2 N 64-bit address adds on the
-// min/max pipe, N cp.async issue slots per lane and day -- ncu capture r2: 59 IADD3 + 30 LDGSTS +
-// 28 FSETP of 545 ALU-pipe instructions per warp-day): the input is described ONCE as a 3-D tensor
+// min/max pipe, N cp.async issue slots per lane and day): the input is described ONCE as a 3-D tensor
 // (cell, day-of-year, year) and a dedicated producer warp issues ONE bulk tensor copy per day --
 // box 128 cells x 1 day x N years -> the [N][128] staging tile -- against an mbarrier; the four
 // consumer warps only wait, read their column (conflict-free LDS) and run the networks.  A window
@@ -1067,7 +1066,7 @@ int32_t launch_generic(const float* x, int64_t T, int64_t C, int64_t ldx, const 
   if (nd <= 0) return XC_OK;
   const int64_t cblocks = (C + kThreads - 1) / kThreads;
   // enough chunks to fill the machine when the grid is narrow
-  int chunks = (int)((148 * 8 + cblocks - 1) / cblocks);
+  int chunks = (int)((sm_count() * 8 + cblocks - 1) / cblocks);
   chunks = chunks < 1 ? 1 : (chunks > nd ? nd : chunks);
   const int per = (nd + chunks - 1) / chunks;
   chunks = (nd + per - 1) / per;
@@ -1086,7 +1085,7 @@ int32_t launch_uniform(const float* x, int64_t T, int64_t C, int64_t ldx, int32_
   const int nd = d_end - d_begin;
   if (nd <= 0) return XC_OK;
   const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  int chunks = (int)((148 * 12 + cblocks - 1) / cblocks);
+  int chunks = (int)((sm_count() * 12 + cblocks - 1) / cblocks);
   chunks = chunks < 1 ? 1 : chunks;
   int per = (nd + chunks - 1) / chunks;
   if (per < 8 * W) per = 8 * W;  // keep the halo overhead (W-1 extra day lists per chunk) small
@@ -1118,7 +1117,7 @@ int32_t launch_w5(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t L, 
   const int nd = d_end - d_begin;
   if (nd <= 0) return XC_OK;
   const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  int chunks = (int)((148 * 16 + cblocks - 1) / cblocks);
+  int chunks = (int)((sm_count() * 16 + cblocks - 1) / cblocks);
   chunks = chunks < 1 ? 1 : chunks;
   int per = (nd + chunks - 1) / chunks;
   if (per < 40) per = 40;  // 4 extra day lists per chunk
@@ -1181,7 +1180,7 @@ int32_t launch_w5_tma(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t
   if (r != CUDA_SUCCESS) return 1;
   const int nd = L;
   const int64_t cblocks = (C + kTmaCells - 1) / kTmaCells;
-  int chunks = (int)((148 * 12 + cblocks - 1) / cblocks);
+  int chunks = (int)((sm_count() * 12 + cblocks - 1) / cblocks);
   chunks = chunks < 1 ? 1 : chunks;
   int per = (nd + chunks - 1) / chunks;
   if (per < 40) per = 40;  // 4 extra day lists per chunk
@@ -1300,7 +1299,7 @@ static int32_t percentile_doy_impl(const float* x, int64_t T, int64_t C, int64_t
         XC_CHECK_CUDA(cudaFuncSetAttribute(percentile_doy_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)smem));
       const int64_t cblocks = (C + kSelThreads - 1) / kSelThreads;
-      int chunks = (int)((148 * 8 + cblocks - 1) / cblocks);
+      int chunks = (int)((sm_count() * 8 + cblocks - 1) / cblocks);
       chunks = chunks < 1 ? 1 : (chunks > n_doy ? n_doy : chunks);
       const int per_chunk = (n_doy + chunks - 1) / chunks;
       chunks = (n_doy + per_chunk - 1) / per_chunk;

@@ -9,7 +9,7 @@
 //   indices/generic.py:83-125       select_resample_op ; 1514-1552 cumulative_difference
 //   core/missing.py:296-322         MissingAny's valid-step count (fused as `valid_count`)
 //
-// Design (B200): the (time, lat, lon) buffer is coalesced along cells, so a THREAD owns VEC=4
+// Design: the (time, lat, lon) buffer is coalesced along cells, so a THREAD owns VEC=4
 // adjacent cells (one 128-bit load per time step; a warp reads 512 contiguous bytes per step) and
 // marches through the time steps of ONE period keeping the run-length state machine in
 // registers -- no shuffles, no shared memory, no intermediate arrays.  The grid is
@@ -456,15 +456,13 @@ __device__ __forceinline__ T pick_uniform(const T (&a)[N], int j) {
   return r;
 }
 
-// Pipe balance (sm_100a issues one warp instruction per clock but the ALU pipe -- compares, selects, integer
+// Pipe balance (an SM sub-partition issues one warp instruction per clock but the ALU pipe -- compares, selects, integer
 // adds, min/max -- and the FMA pipe each take one every OTHER clock): run lengths and counters are kept as
 // float32 (exact below 2^24 steps) so that their updates are FFMA / FADD on the FMA pipe,
 //     cf = (sgn * v > thr) ? 1 : 0;   len' = cf * len + cf;   fin = len - cf * len;   n += cf
 // leaving one FSET and one FMNMX per condition on the ALU pipe, and the run outputs sit at fixed places (two
-// per leading condition) so that no select chain is needed to find their condition.  History (tasmax pass of
-// the batch, quarter grid, HBM time 1.75 ms): integer state, 4 cells per thread 19.1 ms (255 registers);
-// unit list + 2 cells 15.4 ms; float state 13.3 ms (ncu: ALU pipe 74 %, 18 FSEL + 18 ISETP per element in
-// the select chains, long_scoreboard 50 % at 16 warps per SM).
+// per leading condition) so that no select chain is needed to find their condition.  (Integer state with 4 cells
+// per thread needed 255 registers; integer state spends 18 FSEL + 18 ISETP per element in the select chains.)
 // VEC / UNROLL: light passes (no run outputs) take 4 cells per thread, the others 2 cells and more rows in flight.
 template <int NC, int NCR, int NM, int NS, int VEC, int UNROLL>
 __global__ void __launch_bounds__(kThreads)

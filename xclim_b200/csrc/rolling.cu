@@ -7,7 +7,7 @@
 //   indices/generic.py:434-540   spell_mask, general path (:519-535) and min/max fast path (:503-518)
 //   indices/generic.py:543-585   _spell_length_statistics (window > 1)
 //
-// Design (B200): a lane owns one cell and walks the time steps of one period; the w values of a
+// Design: a lane owns one cell and walks the time steps of one period; the w values of a
 // window are re-read from L1/L2 (the rows were just fetched by the same warp), so DRAM traffic stays
 // one read of the input.  These are the low-volume members of the family (the window == 1 fast
 // kernels in period_stats.cu carry the headline configurations); operators are runtime switches.

@@ -17,7 +17,7 @@ from ._lib import check, load
 
 def _require_cuda():
     if not torch.cuda.is_available():
-        raise _lib.XclimB200Error("xclim_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise _lib.XclimB200Error("xclim_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
 
 
 def current_stream_ptr() -> int:

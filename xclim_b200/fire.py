@@ -1,4 +1,4 @@
-"""B200 implementation behind ``xclim.indices.fire`` (Canadian Forest Fire Weather Index System).
+"""CUDA implementation behind ``xclim.indices.fire`` (Canadian Forest Fire Weather Index System).
 
 SURVEY.md section 8(f).4.  The reference runs ``_fire_weather_calc`` (indices/fire/_cffwis.py:680-873) -- a
 Python loop over days around numba ufuncs -- per dask chunk through ``xr.apply_ufunc``
@@ -333,7 +333,7 @@ def fire_season(tas, snd=None, method="WF93", freq=None, temp_start_thresh="12 d
                 temp_condition_days=3, snow_condition_days=3, snow_thresh="0.01 m"):
     """Fire season mask -- indices/fire/_cffwis.py:1609-1691 (every season, ``freq=None``)."""
     if freq is not None:
-        raise NotImplementedError("fire_season(freq=...) (longest season per period) is not part of the B200 hot path")
+        raise NotImplementedError("fire_season(freq=...) (longest season per period) is not part of the xclim_b200 hot path")
     if not all(np.isscalar(v) for v in (temp_start_thresh, temp_end_thresh, snow_thresh)):
         raise ValueError("Thresholds must be scalar.")
     if method not in ("WF93", "LA08", "GFWED"):

@@ -1,4 +1,4 @@
-"""B200 implementations behind the signatures of ``xclim.indices.generic``.
+"""CUDA implementations behind the signatures of ``xclim.indices.generic``.
 
 Each function keeps the reference's name, argument meaning and error behaviour (cited below) but
 runs as ONE streaming CUDA kernel over the ``(time, lat, lon)`` float32 buffer.
@@ -148,7 +148,7 @@ def domain_count(da, low, high, freq):
 def select_resample_op(da, op, freq="YS", out_units=None, **indexer):
     """Per-period reduction -- indices/generic.py:83-125 (string ops only)."""
     if not isinstance(op, str) or op not in _lib.STATS:
-        raise NotImplementedError(f"resample op {op!r} is not supported by the B200 hot path")
+        raise NotImplementedError(f"resample op {op!r} is not supported by the xclim_b200 hot path")
     x2d, cell_shape, other, ta = _unwrap(da, indexer)
     out, _ = device.period_reduce(x2d, ta.period_offsets(freq), _lib.STATS[op])
     attrs = attrs_of(da)
@@ -212,7 +212,7 @@ def spell_length_statistics(data, threshold, window, win_reducer, op, spell_redu
     outs = []
     for sr in reducers:
         if sr not in _lib.RL_REDUCERS:
-            raise NotImplementedError(f"spell reducer {sr!r} is not supported by the B200 hot path")
+            raise NotImplementedError(f"spell reducer {sr!r} is not supported by the xclim_b200 hot path")
         if gap_mask is not None:
             out = device.period_runstat_gap(gap_mask, poff, _lib.OPS[">"], 0.5, _lib.RL_REDUCERS[sr], min_gap)
         elif sel_mask is not None:
@@ -239,9 +239,9 @@ def select_rolling_resample_op(da, op, window, window_center=True, window_op="me
     """Rolling window statistic, then per-period reduction -- indices/generic.py:128-174."""
     wop = window_op.replace("integral", "sum")
     if wop not in ("sum", "mean", "min", "max"):
-        raise NotImplementedError(f"rolling window_op {window_op!r} is not supported by the B200 hot path")
+        raise NotImplementedError(f"rolling window_op {window_op!r} is not supported by the xclim_b200 hot path")
     if not isinstance(op, str) or op not in _lib.STATS:
-        raise NotImplementedError(f"resample op {op!r} is not supported by the B200 hot path")
+        raise NotImplementedError(f"resample op {op!r} is not supported by the xclim_b200 hot path")
     x2d, cell_shape, other, ta = _unwrap(da)
     if indexer:
         # the reference selects AFTER rolling (indices/generic.py:169-174): rolling on the full series, then

@@ -94,7 +94,7 @@ def days_over_precip_thresh(pr, pr_per, thresh="1 mm/day", freq="YS", bootstrap=
     from .generic import _unwrap, _wrap_periods
 
     if bootstrap:
-        raise NotImplementedError("days_over_precip_thresh(bootstrap=True) is not supported by the B200 hot path")
+        raise NotImplementedError("days_over_precip_thresh(bootstrap=True) is not supported by the xclim_b200 hot path")
     code = _lib.op_code(op, (">", ">="))
     thr = threshold_in_units_of(thresh, pr) if isinstance(thresh, str) else float(thresh)
     x2d, cell_shape, other, ta = _unwrap(pr)
@@ -634,7 +634,7 @@ def multiday_temperature_swing(tasmin, tasmax, thresh_tasmin="0 degC", thresh_ta
     from .field import attrs_of
     from .generic import _unwrap, _wrap_periods
     if op not in _lib.RL_REDUCERS:
-        raise NotImplementedError(f"op {op!r} is not supported by the B200 hot path")
+        raise NotImplementedError(f"op {op!r} is not supported by the xclim_b200 hot path")
     c1 = _lib.op_code(op_tasmin, ("<", "<="))
     c2 = _lib.op_code(op_tasmax, (">", ">="))
     t1 = threshold_in_units_of(thresh_tasmin, tasmin) if isinstance(thresh_tasmin, str) else float(thresh_tasmin)

@@ -64,7 +64,7 @@ def missing_wmo(da, freq, nm=11, nc=5, src_timestep="D", **indexer):
     missing or >= nc consecutive days are missing; a coarser period is missing when any of its months
     is (or when it does not hold all its months)."""
     if indexer:
-        raise NotImplementedError("select_time indexers are outside the B200 hot path")
+        raise NotImplementedError("select_time indexers are outside the xclim_b200 hot path")
     if not (nm < 31 and nc < 31):
         raise ValueError("Options (nm, nc) are invalid for missing method MissingWMO.")
     if src_timestep != "D":

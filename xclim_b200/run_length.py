@@ -1,4 +1,4 @@
-"""B200 implementations behind the signatures of ``xclim.indices.run_length``.
+"""CUDA implementations behind the signatures of ``xclim.indices.run_length``.
 
 The reference functions take a boolean (or 0/1 float) mask ``da`` and a ``freq``; here the mask is
 streamed once through the fused run-length kernel with the condition ``da > 0`` (``rle`` treats
@@ -30,7 +30,7 @@ def _run_reduce(x2d, poff, reducer, window, resample_before_rl):
     if isinstance(reducer, str) and reducer.startswith("q") and reducer[1:].isdigit():
         return device.period_run_quantile(x2d, poff, _GT, 0.0, float(f"0.{reducer[1:]}"), window, resample_before_rl)
     if reducer not in _lib.RL_REDUCERS:
-        raise NotImplementedError(f"reducer {reducer!r} is not supported by the B200 hot path")
+        raise NotImplementedError(f"reducer {reducer!r} is not supported by the xclim_b200 hot path")
     out, _ = device.period_runstat(x2d, poff, _GT, 0.0, _lib.RL_REDUCERS[reducer], window, resample_before_rl)
     return out
 

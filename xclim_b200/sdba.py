@@ -1,4 +1,4 @@
-"""B200 implementation behind ``xclim.sdba.EmpiricalQuantileMapping`` (xsdba; PARITY UNPINNED).
+"""CUDA implementation behind ``xclim.sdba.EmpiricalQuantileMapping`` (xsdba; PARITY UNPINNED).
 
 ``xclim.sdba`` is a shim over the third-party ``xsdba`` package (sdba.py:11) whose sources are not
 part of the reference tree; the algorithm below follows its published behaviour and the reference's
@@ -34,7 +34,7 @@ class EmpiricalQuantileMapping:
     @classmethod
     def train(cls, ref, hist, *, nquantiles=20, kind="+", group="time", **kwargs):
         if group != "time":
-            raise NotImplementedError("only group='time' is part of the B200 hot path")
+            raise NotImplementedError("only group='time' is part of the xclim_b200 hot path")
         if kwargs:
             raise NotImplementedError(f"unsupported training options: {sorted(kwargs)}")
         if kind not in _KINDS:

@@ -172,7 +172,7 @@ class TimeAxis:
         elif base == "D":
             gid = np.arange(len(self), dtype=np.int64)
         else:
-            raise NotImplementedError(f"frequency {freq!r} is not supported by the B200 hot path")
+            raise NotImplementedError(f"frequency {freq!r} is not supported by the xclim_b200 hot path")
         if mult != 1:
             gid = np.floor_divide(gid - gid[0], mult) if gid.size else gid
         return gid
