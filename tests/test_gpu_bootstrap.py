@@ -3,7 +3,7 @@ import numpy as np
 import pytest
 
 from oracle import xclim_oracle as O
-from xb_helpers import make_field
+from xb_helpers import make_field, plant_infinite_samples
 
 pytestmark = pytest.mark.gpu
 
@@ -89,6 +89,17 @@ def test_bootstrap_standard_calendar_365_366_blocks(cuda, per, op, freq):
     np.testing.assert_array_equal(got.values[outside], plain[outside])
 
 
+def _raw_doy_table(x, year, doy, window, pers):
+    """(n_per, 366, C) day-of-year quantiles of O.percentile_doy before its 365 -> 366 re-interpolation"""
+    rr = O.rolling_construct_center(x, window)
+    ny = int(year.max()) + 1
+    rrr = np.full((366, ny * window) + x.shape[1:], np.nan, dtype=rr.dtype)
+    for t in range(x.shape[0]):
+        rrr[doy[t] - 1, year[t] * window:(year[t] + 1) * window] = rr[t]
+    q = np.stack([O.nan_quantile(rrr[d], np.asarray(pers) / 100.0, 1 / 3, 1 / 3) for d in range(366)])
+    return np.moveaxis(q, 1, 0)
+
+
 def test_percentile_vrow_identity_and_replacement(cuda):
     """xc_percentile_doy_vrow_f32: the identity map reproduces the plain table bit for bit, and a block
     replacement equals the table of a physically modified copy of the series."""
@@ -96,13 +107,15 @@ def test_percentile_vrow_identity_and_replacement(cuda):
     import torch
     rng = np.random.default_rng(34)
     T = 366 + 365 * 3 + 366
-    x = _tas(rng, T, (7,), nan_frac=0.01)
+    x = _tas(rng, T, (17,), nan_frac=0.01)
+    plant_infinite_samples(x, [0.9, 0.1], range(7, 17), seed=34)
     da = make_field(x, "2000-01-01", calendar="standard", units="K")
     ta = da.time
     years = np.unique(ta.year)
     yidx = np.searchsorted(years, ta.year).astype(np.int16)
     xd = torch.from_numpy(x).cuda()
     plain = dv.percentile_doy(xd, ta.doy, yidx, 366, len(years), 5, [90.0, 10.0], 1 / 3, 1 / 3)
+    np.testing.assert_array_equal(plain.cpu().numpy(), _raw_doy_table(x, yidx, ta.doy, 5, [90.0, 10.0]))
     ident = dv.percentile_doy(xd, ta.doy, yidx, 366, len(years), 5, [90.0, 10.0], 1 / 3, 1 / 3,
                               vrow=np.arange(T, dtype=np.int32))
     assert torch.equal(plain.view(torch.int64), ident.view(torch.int64))
@@ -116,6 +129,7 @@ def test_percentile_vrow_identity_and_replacement(cuda):
     got = dv.percentile_doy(xd, ta.doy, yidx, 366, len(years), 5, [90.0], 1 / 3, 1 / 3, vrow=vrow)
     ref = dv.percentile_doy(torch.from_numpy(z).cuda(), ta.doy, yidx, 366, len(years), 5, [90.0], 1 / 3, 1 / 3)
     assert torch.equal(got.view(torch.int64), ref.view(torch.int64))
+    np.testing.assert_array_equal(got.cpu().numpy(), _raw_doy_table(z, yidx, ta.doy, 5, [90.0]))
     # year 2000 (366 days, rows 0..365) <- year 2002 with NaN on Feb 29
     src0 = 366 + 365
     rows = np.insert(src0 + np.arange(365), 59, -1)

@@ -3,7 +3,7 @@ import numpy as np
 import pytest
 
 from oracle import xclim_oracle as O
-from xb_helpers import make_field
+from xb_helpers import make_field, plant_infinite_samples
 
 pytestmark = pytest.mark.gpu
 
@@ -36,6 +36,7 @@ def test_percentile_doy_uniform_calendars(cuda, calendar, years, per):
     x = _tas(rng, T, shape)
     x[:, 0, 0] = np.nan          # an all-NaN cell
     x[5:400, 0, 1] = np.nan      # a long gap
+    plant_infinite_samples(x, [per / 100], range(40, 45), seed=years)
     da = make_field(x, "1981-01-01", calendar=calendar, units="K")
     got = xcal.percentile_doy(da, window=5, per=per)
     exp = O.percentile_doy(x, da.time.year, da.time.doy, 5, per)[:, 0]
@@ -58,6 +59,7 @@ def test_percentile_doy_windows_and_types(cuda, window):
     from xclim_b200 import calendar as xcal
     rng = np.random.default_rng(12)
     x = _tas(rng, 365 * 8, (4, 4))
+    plant_infinite_samples(x, [0.05, 0.95], range(6, 16), seed=window)
     da = make_field(x, "1990-01-01", calendar="noleap", units="K")
     for alpha, beta in ((1 / 3, 1 / 3), (1.0, 1.0), (0.0, 1.0)):
         got = xcal.percentile_doy(da, window=window, per=[5.0, 95.0], alpha=alpha, beta=beta)
@@ -171,12 +173,14 @@ def test_doy_count_year_blocked_kernel_exact_ties(cuda, op):
 def test_percentile_doy_mid_percentiles_selection_kernel(cuda, calendar, years, window):
     """Percentiles whose order statistics are more than 64 ranks from both ends of the sample (the
     median of 150 values ...) go through the selection kernel; a list of percentiles mixes it with the
-    network kernels.  Heavy ties, NaNs, an all-NaN cell and a single-value cell included."""
+    network kernels.  Heavy ties, NaNs, an all-NaN cell, a single-value cell and infinite samples included."""
     from xclim_b200 import calendar as xcal
     rng = np.random.default_rng(13)
     L = {"noleap": 365, "standard": 365.25, "360_day": 360}[calendar]
     T = int(years * L)
-    x = _tas(rng, T, (3, 5), nan_frac=0.02)
+    x = _tas(rng, T, (6, 5), nan_frac=0.02)
+    if calendar != "standard":   # (the 365 -> 366 re-interpolation of such tables is not covered here)
+        plant_infinite_samples(x, [0.5, 0.1, 0.9], range(15, 30), seed=years)
     x[:, 0, 0] = np.nan
     x[:, 0, 1] = np.round(x[:, 0, 1])            # ties
     x[:, 0, 2] = np.where(rng.random(T) < 0.5, 0.0, -0.0).astype(np.float32)  # signed zeros only
@@ -197,7 +201,8 @@ def test_percentile_doy_mid_percentiles_selection_kernel(cuda, calendar, years, 
 def test_percentile_doy_tma_path(cuda, years, per, monkeypatch):
     """The TMA-fed window-5 kernel (30..32 uniform years, ldx % 4 == 0): bit-exact vs the oracle and vs
     the lane-by-lane kernel, with NaNs, infinities of both signs (the FADD NaN probe's false positive),
-    cells beyond the last full 128-cell tile, and windows that reach into the neighbouring year."""
+    cells beyond the last full 128-cell tile, windows that reach into the neighbouring year, and samples
+    whose interpolation meets infinities or overflows (NaN lerp -> the sample maximum)."""
     import torch
     from xclim_b200 import device
     rng = np.random.default_rng(100 + years)
@@ -209,6 +214,7 @@ def test_percentile_doy_tma_path(cuda, years, per, monkeypatch):
     x[7, 1, 2], x[365 + 7, 1, 2] = np.inf, -np.inf        # same day of year: inf + (-inf) = NaN in the probe
     x[0:3, 2, 3] = np.nan                                 # first days of the series
     x[T - 2:, 2, 4] = np.nan                              # last days
+    plant_infinite_samples(x, [per / 100], list(range(60, 63)) + [138, 139], seed=years)
     doy = (np.arange(T) % L + 1).astype(np.int16)
     yidx = (np.arange(T) // L).astype(np.int16)
     xd = torch.from_numpy(x.reshape(T, -1)).cuda()

@@ -11,3 +11,28 @@ def make_field(values, start="2000-01-01", calendar="standard", units="K", dims=
     if dims is None:
         dims = ("time",) + tuple(f"d{i}" for i in range(values.ndim - 1))
     return Field(values, dims, ta, {}, {"units": units, **attrs})
+
+
+def plant_infinite_samples(x, qs, cells, seed=0):
+    """Overwrite five cells per quantile q of ``x`` (time first; ``cells`` are flat cell indexes, used in
+    order) with infinite or overflowing values placed around the q-quantile's neighbours, so that the
+    interpolation meets +inf at the top ranks, a -inf left neighbour, the pair {-inf, +inf} (also in
+    two-value samples) and finite +-3e38 whose difference overflows float32.  Returns the cells used."""
+    rng = np.random.default_rng(seed)
+    flat = x.reshape(x.shape[0], -1)
+    assert np.shares_memory(flat, x)
+    T = x.shape[0]
+    big = np.float32(3e38)
+    used = []
+    it = iter(cells)
+    for q in qs:
+        u = rng.random(T)
+        c = next(it); flat[u < 1.1 * (1 - q), c] = np.inf; used.append(c)          # +inf at the top ranks
+        c = next(it); flat[u < 1.1 * q, c] = -np.inf; used.append(c)               # -inf left neighbours
+        c = next(it); flat[:, c] = np.where(u < q, -np.inf, np.inf); used.append(c)  # {-inf, +inf}
+        v = np.where(rng.random(T) < 0.5, -np.inf, np.inf)
+        c = next(it); flat[:, c] = np.where(rng.random(T) < 0.985, np.nan, v); used.append(c)
+        c = next(it); used.append(c)                                                # +-3e38 and +inf next to -3e38
+        flat[:, c] = np.where(u < 0.9 * q, -big, np.where(u > 1 - 0.9 * (1 - q), big, flat[:, c]))
+        flat[(u > 0.5 * q) & (u < 0.5 * q + 0.05), c] = np.inf
+    return used

@@ -54,6 +54,50 @@ __device__ __forceinline__ void remove_one(float (&a)[K], float r) {
   a[K - 1] = found ? XC_NEG_INF : a[K - 1];
 }
 
+// The rank shortcuts of both kernels count "x beats the threshold" on the selection side, which is the
+// operator's side only for >, >= with the top list and <, <= with the bottom one; any other pairing (a tx90p
+// count against a low percentile) evaluates every year exactly.  They also assume that the threshold of every
+// altered sample lies between its two neighbours.  An infinite neighbour, or two neighbours whose difference overflows float32, breaks that (the
+// lerp can give +-inf, or NaN -> the sample maximum), so such a day sends every year through the exact
+// per-(y, s) evaluation.  On interior days every neighbour is among the min(nbase, K) values at the top of tl
+// (the selection side of S(d)); near the ends of the year block s can bring in a value from outside S(d), so
+// there the whole raw window ([W][N] rows `stride` apart from `raw`) is checked.
+template <int OP>
+__device__ __forceinline__ bool rank_side(bool top) {
+  return top == (OP == XC_OP_GT || OP == XC_OP_GE);
+}
+// interior days: hi = tl[0], lo = the last valid entry of tl
+__device__ __forceinline__ bool span_overflows(float hi, float lo) { return !isfinite(__fsub_rn(hi, lo)); }
+// days near the ends of the year ([count] values `stride` apart); out of line to keep the kernels' registers
+__device__ __noinline__ bool raw_span_overflows(const float* raw, int stride, int count) {
+  float hi = XC_NEG_INF, lo = -XC_NEG_INF;
+  for (int i = 0; i < count; ++i) {
+    const float v = raw[(size_t)i * stride];
+    hi = fmaxf(hi, v);
+    lo = fminf(lo, v);
+  }
+  return span_overflows(hi, lo);
+}
+
+// Largest value of the altered sample M(y, s, d): the window values of every block but y, plus block s's at
+// the positions y contributes (vmask) -- the NaN-interpolation fallback (lerp_is_nan), rarely taken.  raw:
+// this lane's [W][N] ring (rows `stride` apart, slot of day d-H = raw_first) holding sgn * x.
+__device__ __noinline__ float altered_max(const float* raw, int stride, int raw_first, int W, int N, int L, int d,
+                                          int y, int s, unsigned vmask, float sgn) {
+  const int H = W / 2;
+  float m = XC_NEG_INF;
+  for (int k = 0; k < W; ++k) {
+    const int e = d - H + k;
+    const float* row = raw + (size_t)((raw_first + k) % W) * N * stride;
+    for (int b = 0; b < N; ++b) {
+      const bool valid = (e < 0) ? (b + 1 < N) : ((e >= L) ? (b >= 1) : true);
+      if (valid && b != y) m = fmaxf(m, sgn * row[(size_t)b * stride]);
+    }
+    if ((vmask >> k) & 1u) m = fmaxf(m, sgn * row[(size_t)s * stride]);
+  }
+  return m;
+}
+
 // Shared-memory layout per lane (column `lane` of every row):
 //   sring [W-1][KA]  sorted (selection-side, masked) extremes of the W-1 previous day lists
 //   scnt  [W-1]      their valid counts
@@ -114,6 +158,7 @@ bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t ba
     }
   };
 
+  int raw_first = 0;  // raw-ring slot of day d-H
   float ynew[KA];
   int nnew;
   // prologue: days e = d0-H .. d0+H-1 ; sorted slot = (e - (d0-H)) mod R, raw slot = (e - (d0-H)) mod W
@@ -124,7 +169,6 @@ bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t ba
     scnt[s * kThreads + lane] = nnew;
   }
   int oldest = 0;     // sorted-ring slot of day d-H
-  int raw_first = 0;  // raw-ring slot of day d-H
   for (int d = d0; d < d1; ++d) {
     const int raw_new = (raw_first + W - 1) % W;
     load_day(d + H, raw_new, ynew, nnew);
@@ -140,6 +184,9 @@ bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t ba
       bitonic_finish_desc<KA>(tl);
       nbase += scnt[s * kThreads + lane];
     }
+    const bool hostile = !rank_side<OP>(top) ||
+                         ((d >= H) && (d + H < L) ? nbase > 0 && span_overflows(tl[0], pick<KA>(tl, min(nbase, KA) - 1))
+                                                  : raw_span_overflows(raw + lane, kThreads, W * N));
     // ---- every in-base year y: first a cheap, conservative test on ranks.  With M = S - R_y + I_s,
     // ge(M) = #{m >= x} lies in [geA, geA + W] (geA from S - R_y alone) and the two order statistics the
     // quantile interpolates sit at list indexes k1 and k1 + 1:  ge(M) <= k1 for every s  =>  x beats the
@@ -182,7 +229,7 @@ bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t ba
       const int k1min = top ? (na - 2 - q0.ilo) : q0.ilo;
       const int k1max = top ? (na + W - 2 - q1.ilo) : q1.ilo;
       bool decided = false;
-      if (ok0 && ok1 && N <= 32) {
+      if (ok0 && ok1 && N <= 32 && !hostile) {
         if (gtA >= k1max + 2) {
           decided = true;                       // never beats the threshold
         } else if (geT < KA && geA + W <= k1min) {
@@ -239,16 +286,19 @@ bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t ba
           nm += ok ? 1 : 0;
           insert_desc<KB>(bl, ok ? sgn * v : XC_NEG_INF);
         }
-        const double p = finalize_quantile<KB>(bl, nm, spec);
+        double p = finalize_quantile<KB>(bl, nm, spec);
+        if (lerp_is_nan(p, nm)) p = altered_max(raw + lane, kThreads, raw_first, W, N, L, d, y, s, vmask, 1.f);
         cnt += cmpd<OP>((double)xq, p) ? 1 : 0;
       }
       if (cnt) atomicAdd(counts + (int64_t)step_period[y * L + d] * C + c, cnt);
     }
-    // rotate the rings
+    // rotate the rings (window 1 keeps no sorted ring: R == 0 slots)
+    if (R > 0) {
 #pragma unroll
-    for (int k = 0; k < KA; ++k) sring[((size_t)oldest * KA + k) * kThreads + lane] = ynew[k];
-    scnt[oldest * kThreads + lane] = nnew;
-    oldest = (oldest + 1 == R) ? 0 : oldest + 1;
+      for (int k = 0; k < KA; ++k) sring[((size_t)oldest * KA + k) * kThreads + lane] = ynew[k];
+      scnt[oldest * kThreads + lane] = nnew;
+      oldest = (oldest + 1 == R) ? 0 : oldest + 1;
+    }
     raw_first = (raw_first + 1 == W) ? 0 : raw_first + 1;
   }
 }
@@ -406,13 +456,16 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
     for (int b = 0; b < KA; ++b) { y0[b] = y1[b]; y1[b] = y2[b]; y2[b] = y3[b]; y3[b] = ynew[b]; }
     n0 = n1; n1 = n2; n2 = n3; n3 = nnew;
     const bool interior = (d >= H) && (d + H < L);   // the window stays inside the year: every position valid
+    const bool hostile = !rank_side<OP>(top) ||
+                         (interior ? nbase > 0 && span_overflows(tl[0], pick16(tl, min(nbase, KA) - 1))
+                                   : raw_span_overflows(raw + lane, kBT, W * N));
     // ---- day constants: list ranks of the interpolated order statistics over every possible count
     // na in [nbase - W, nbase] of A_y (k1 is non-decreasing in n), cf. the per-year test below
     bool okA, okB, okC;
     const int k1lo = k1_of(nbase - W, okA);            // smallest k1min over the years
     const int k1hi = k1_of(nbase + W, okB);            // largest k1max
     const int k1reg = k1_of(nbase, okC);               // regular item: na + W = nbase
-    const bool day_ok = okA && okB && (nbase - W >= 2);
+    const bool day_ok = okA && okB && (nbase - W >= 2) && !hostile;
     // never: gtA >= k1max + 2  <=  gtT - W >= k1hi + 2  <=  xs < tl[k1hi + W + 1]
     // always: geT < KA and geA + slack <= k1min  <=  geT <= idx with 2 idx <= k1lo (interior) / idx + W <= k1lo
     const int i_never = k1hi + W + 1;
@@ -474,7 +527,7 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
         k1min = k1_of(na, ok0);
         k1max = k1_of(na + W, ok1);
       }
-      ok0 = ok0 && (na >= 2);
+      ok0 = ok0 && (na >= 2) && !hostile;
       // bootstrap_kernel's test on geT = #{tl >= xs}, gtT = #{tl > xs} (tl sorted, counts saturate at KA):
       //   never : gtA >= k1max + 2, gtA = (gtT == KA) ? KA : gtT - gtR   <=>  gtT >= min(KA, k1max + 2 + gtR)
       //                                                               <=>  xs < tl[min(KA, k1max + 2 + gtR) - 1]
@@ -527,7 +580,7 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
       bool okm;
       const int k1 = (nm0 == nbase) ? k1reg : k1_of(nm0, okm);
       if (nm0 == nbase) okm = okC;
-      const bool regular = interior && okm && k1 >= 0 && (k1 + 1 <= KA - 1 - W);
+      const bool regular = interior && !hostile && okm && k1 >= 0 && (k1 + 1 <= KA - 1 - W);
       const QuantIdx qm = quant_index(nm0, spec);
       float b0 = 0.f, b1 = 0.f, b2 = 0.f, b3 = 0.f, b4 = 0.f, b5 = 0.f, b6 = 0.f;
       const unsigned all = (N >= 32) ? ~0u : ((1u << N) - 1u);
@@ -592,7 +645,8 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
           nm += ok ? 1 : 0;
           insert_desc<KB>(bl, ok ? v : XC_NEG_INF);
         }
-        const double p = finalize_quantile<KB>(bl, nm, spec);
+        double p = finalize_quantile<KB>(bl, nm, spec);
+        if (lerp_is_nan(p, nm)) p = altered_max(raw + lane, kBT, raw_first, W, N, L, d, y, s, vmask, sgn);
         cnt += cmpd<OP>((double)xq, p) ? 1 : 0;
       }
       if (cnt) atomicAdd(counts + (int64_t)step_period[y * L + d] * C + c, cnt);

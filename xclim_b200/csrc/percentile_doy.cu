@@ -58,6 +58,46 @@ __device__ __forceinline__ void insert_desc(float (&lst)[K], float v) {
   }
 }
 
+// Largest non-NaN value of the sample of day d, for the NaN-interpolation fallback (lerp_is_nan).
+// Row map of the generic and selection kernels: step i = pos[y * n_doy + d] of year y, steps i-h..i+h,
+// read through vrow when given.
+__device__ __noinline__ float sample_max_steps(const float* col, int64_t T, int64_t ldx, const int32_t* pos,
+                                               int n_doy, int n_years, int h, int d, const int32_t* vrow) {
+  float m = XC_NEG_INF;
+  for (int y = 0; y < n_years; ++y) {
+    const int i = pos[y * n_doy + d];
+    if (i < 0) continue;
+    const int j0 = max(0, i - h), j1 = min((int)T - 1, i + h);
+    for (int j = j0; j <= j1; ++j) {
+      const int row = vrow ? vrow[j] : j;
+      if (row >= 0) m = fmaxf(m, __ldg(col + (int64_t)row * ldx));
+    }
+  }
+  return m;
+}
+
+// The same for the per-day-list kernels: the union of days e = d-h..d+h over the years, rows y*L + e
+// (uniform years; e < 0 / e >= L reach into the neighbouring year) or pos[y * n_doy + e] (table mode).
+template <bool TABLE>
+__device__ __noinline__ float sample_max_days(const float* x, int64_t c, int64_t ldx, int L, int N, int d, int h,
+                                              const int32_t* pos, int n_doy) {
+  float m = XC_NEG_INF;
+  for (int e = d - h; e <= d + h; ++e) {
+    for (int y = 0; y < N; ++y) {
+      int64_t row;
+      if (TABLE) {
+        row = pos[y * n_doy + e];
+        if (row < 0) continue;
+      } else {
+        if ((e < 0 && y == 0) || (e >= L && y == N - 1)) continue;
+        row = (int64_t)y * L + e;
+      }
+      m = fmaxf(m, __ldg(x + row * ldx + c));
+    }
+  }
+  return m;
+}
+
 // ------------------------------------------------------------------------------------------------
 // generic kernel: pos[y * n_doy + (d-1)] = row of (year y, doy d) or -1
 // ------------------------------------------------------------------------------------------------
@@ -90,7 +130,9 @@ percentile_doy_generic_kernel(const float* __restrict__ x, int64_t T, int64_t C,
         insert_desc<K>(lst, v);
       }
     }
-    out[(int64_t)d * C + c] = finalize_quantile<K>(lst, n, spec);
+    double res = finalize_quantile<K>(lst, n, spec);
+    if (lerp_is_nan(res, n)) res = sample_max_steps(col, T, ldx, pos, n_doy, n_years, h, d, vrow);
+    out[(int64_t)d * C + c] = res;
   }
 }
 
@@ -158,7 +200,8 @@ percentile_doy_select_kernel(const float* __restrict__ x, int64_t T, int64_t C, 
       }
       const float left = key_value(v);
       if (single) {
-        res = (double)left;
+        // the clamp to the minimum interpolates between two copies of it: NaN for -inf (see finalize_quantile)
+        res = (n > 1 && qi.vi < 0.0 && isinf(left)) ? __longlong_as_double(0x7ff8000000000000LL) : (double)left;
       } else {
         int le = 0;
         uint32_t nxt = 0xffffffffu;
@@ -170,6 +213,7 @@ percentile_doy_select_kernel(const float* __restrict__ x, int64_t T, int64_t C, 
         const float right = (le >= k + 2) ? left : key_value(nxt);
         res = quant_lerp(left, right, qi);
       }
+      if (lerp_is_nan(res, n)) res = sample_max_steps(col, T, ldx, pos, n_doy, n_years, h, d, vrow);
     }
     out[(int64_t)d * C + c] = res;
   }
@@ -471,7 +515,9 @@ percentile_doy_uniform_kernel(const float* __restrict__ x, int32_t T, int64_t C,
       bitonic_finish_desc<K>(acc);
       n += rcnt[s * kThreads + lane];
     }
-    out[(int64_t)d * C + c] = finalize_quantile<K>(acc, n, spec);
+    double res = finalize_quantile<K>(acc, n, spec);
+    if (lerp_is_nan(res, n)) res = sample_max_days<TABLE>(x, c, ldx, L, N, d, H, pos, n_doy);
+    out[(int64_t)d * C + c] = res;
     // the new list replaces the oldest one
 #pragma unroll
     for (int k = 0; k < K; ++k) ring[((size_t)oldest * K + k) * kThreads + lane] = ynew[k];
@@ -606,6 +652,7 @@ percentile_doy_w5p_kernel(const float* __restrict__ x, int32_t T, int64_t C, int
       bitonic_finish_desc<K>(u);
       res = finalize_quantile<K>(u, n, spec);
     }
+    if (lerp_is_nan(res, n)) res = sample_max_days<TABLE>(x, c, ldx, L, N, day, 2, pos, n_doy);
     out[(int64_t)day * C + c] = res;
   }
 }
@@ -702,7 +749,8 @@ __device__ __forceinline__ void finish_chunk_t(bool top, float (&v)[K], int& nv)
 template <int N2>   // years = 16 + N2, N2 in {14, 15, 16}
 __global__ void __launch_bounds__(kTmaThreads, XC_PCTL_TMA_MINBLOCKS)
 percentile_doy_w5t_kernel(const __grid_constant__ CUtensorMap tmap, int64_t C, int32_t L, QuantSpec spec,
-                          int32_t doys_per_chunk, double* __restrict__ out, int32_t d_begin, int32_t d_end) {
+                          int32_t doys_per_chunk, double* __restrict__ out, int32_t d_begin, int32_t d_end,
+                          const float* __restrict__ x, int64_t ldx) {
   constexpr int K = 16;
   constexpr int N = K + N2;
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -834,6 +882,8 @@ percentile_doy_w5t_kernel(const __grid_constant__ CUtensorMap tmap, int64_t C, i
       bitonic_finish_desc<K>(u);
       res = finalize_quantile<K>(u, n, spec);
     }
+    // cells beyond C hold the NaN fill (n == 0) and never reach the fallback's global reads
+    if (lerp_is_nan(res, n)) res = sample_max_days<false>(x, c, ldx, L, N, day, 2, nullptr, 0);
     if (c < C) out[(int64_t)day * C + c] = res;
   }
 }
@@ -1192,7 +1242,7 @@ int32_t launch_w5_tma(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t
   auto go = [&](auto kern) -> int32_t {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(percentile_doy_w5t_kernel)");
-    kern<<<grid, kTmaThreads, smem, st>>>(map, C, L, spec, per, out, 0, L);
+    kern<<<grid, kTmaThreads, smem, st>>>(map, C, L, spec, per, out, 0, L, x, ldx);
     return launch_status("percentile_doy_w5t_kernel");
   };
   if (N == 30) return go(percentile_doy_w5t_kernel<14>);

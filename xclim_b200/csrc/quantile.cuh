@@ -66,7 +66,9 @@ __device__ __forceinline__ double finalize_quantile(const float (&lst)[K], int n
   if (s.top) {
     if (vi >= nd - 1.0) return (double)lst[0];
   } else {
-    if (vi < 0.0) return (double)(-lst[0]);
+    // both neighbours clamp to the minimum; for a -inf minimum their difference is NaN, which the caller
+    // replaces by the sample maximum (lerp_is_nan)
+    if (vi < 0.0) return isinf(lst[0]) ? __longlong_as_double(0x7ff8000000000000LL) : (double)(-lst[0]);
   }
   const double lo = floor(vi);
   const int ilo = (int)lo;
@@ -108,5 +110,11 @@ __device__ __forceinline__ double quant_lerp(float left, float right, const Quan
   if (g >= 0.5) return __dadd_rn((double)right, -__dmul_rn((double)diff, __dadd_rn(1.0, -g)));
   return __dadd_rn((double)left, __dmul_rn((double)diff, g));
 }
+
+// core/utils.py:554: an interpolation that comes out NaN (an infinite neighbour, or two neighbours whose
+// difference overflows float32) is replaced by the largest value of the sample.  With n >= 2 values a NaN
+// result can only come from there, so the kernels test the result after the lerp and only then look the
+// maximum up (the bottom-side lists do not hold it).
+__device__ __forceinline__ bool lerp_is_nan(double r, int n) { return n >= 2 && r != r; }
 
 }  // namespace xc
