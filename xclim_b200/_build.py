@@ -50,29 +50,6 @@ def _deps_mtime() -> float:
     return max(os.path.getmtime(h) for h in hdrs)
 
 
-def build_variant(tag: str, defines: list[str]) -> str:
-    """Experiment helper: a second library `libxclim_b200_<tag>.so` compiled with extra -D flags
-    (select it at run time with XCLIM_B200_LIB=<path>).  Not part of the product build."""
-    nvcc = _nvcc()
-    out = os.path.join(LIB_DIR, f"libxclim_b200_{tag}.so")
-    odir = os.path.join(ROOT, "build", f"obj_{tag}")
-    os.makedirs(odir, exist_ok=True)
-    objs = []
-    for src in sources():
-        obj = os.path.join(odir, os.path.basename(src)[:-3] + ".o")
-        r = subprocess.run([nvcc, *NVCC_FLAGS, *EXTRA_FLAGS.get(os.path.basename(src), []),
-                            *[f"-D{d}" for d in defines], "-c", src, "-o", obj],
-                           capture_output=True, text=True)
-        if r.returncode != 0:
-            raise RuntimeError(r.stderr)
-        objs.append(obj)
-    r = subprocess.run([nvcc, "-shared", *ARCH_FLAGS, "-o", out, *objs],
-                       capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(r.stderr)
-    return out
-
-
 def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(OBJ_DIR, exist_ok=True)
     os.makedirs(LIB_DIR, exist_ok=True)

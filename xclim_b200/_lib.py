@@ -130,12 +130,11 @@ def load() -> C.CDLL:
     global _lib
     if _lib is not None:
         return _lib
-    path = os.environ.get("XCLIM_B200_LIB") or LIB_PATH   # XCLIM_B200_LIB: experiment builds only
-    if not os.path.exists(path):
+    if not os.path.exists(LIB_PATH):
         raise XclimB200Error(
-            f"{path} is missing: build it with `python -m xclim_b200._build` "
+            f"{LIB_PATH} is missing: build it with `python -m xclim_b200._build` "
             "(the xclim_b200 hot path has no CPU fallback)")
-    lib = C.CDLL(path)
+    lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)
         fn.restype = res

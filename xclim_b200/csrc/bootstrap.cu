@@ -29,17 +29,6 @@ namespace xc {
 namespace {
 
 constexpr int kThreads = 128;
-#define XC_NEG_INF (__int_as_float(0xff800000))
-
-template <int K>
-__device__ __forceinline__ void insert_desc(float (&lst)[K], float v) {
-#pragma unroll
-  for (int k = 0; k < K; ++k) {
-    const float hi = fmaxf(lst[k], v);
-    v = fminf(lst[k], v);
-    lst[k] = hi;
-  }
-}
 
 // remove ONE instance of value r from the sorted list (no-op when absent; NaN never matches)
 template <int K>
@@ -329,10 +318,7 @@ bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t ba
 // (544 bytes for N = 15: the sorted day lists are rebuilt from the raw ring instead of being kept, which
 // trades 7 % more instructions for 50 % more resident warps in a latency-bound kernel).  N <= 16.
 // ------------------------------------------------------------------------------------------------
-#ifndef XC_BOOT_THREADS
-#define XC_BOOT_THREADS 32
-#endif
-constexpr int kBT = XC_BOOT_THREADS;
+constexpr int kBT = 32;   // threads per CTA: one warp
 constexpr float kPosInf = __builtin_huge_valf();
 
 __device__ __forceinline__ void sort5_desc(float& a, float& b, float& c, float& d, float& e) {
@@ -658,22 +644,17 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
 int32_t launch_bootstrap5(int32_t op, const float* x, int64_t C, int64_t ldx, int64_t base_start, int32_t N, int32_t L,
                           const QuantSpec& spec, const int32_t* step_period, int32_t* counts, cudaStream_t st) {
   const int64_t cblocks = (C + kBT - 1) / kBT;
-  int chunks = (int)((sm_count() * 12 + cblocks - 1) / cblocks);
-  chunks = chunks < 1 ? 1 : chunks;
-  int per = (L + chunks - 1) / chunks;
-  if (per < 20) per = 20;
-  if (per > L) per = L;
-  chunks = (L + per - 1) / per;
+  const DaySplit sp = split_days(L, cblocks, 12, 20, false);
   const size_t smem = ((size_t)8 * N + 16) * kBT * 4;
   if (smem > 227 * 1024) return 1;
-  dim3 grid((unsigned)cblocks, (unsigned)chunks, 1);
+  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
   return dispatch_op(op, [&](auto OPC) -> int32_t {
     constexpr int OP = decltype(OPC)::value;
     if (smem > 48 * 1024) {
       cudaError_t e = cudaFuncSetAttribute(bootstrap5_kernel<OP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(bootstrap5_kernel)");
     }
-    bootstrap5_kernel<OP><<<grid, kBT, smem, st>>>(x, C, ldx, base_start, N, L, spec, step_period, per, counts);
+    bootstrap5_kernel<OP><<<grid, kBT, smem, st>>>(x, C, ldx, base_start, N, L, spec, step_period, sp.per, counts);
     return launch_status("bootstrap5_kernel");
   });
 }
@@ -689,18 +670,13 @@ int32_t launch_bootstrap(int32_t op, const float* x, int64_t C, int64_t ldx, int
                          int32_t L, int32_t W, const QuantSpec& spec, const int32_t* step_period, int32_t* counts,
                          cudaStream_t st) {
   const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  int chunks = (int)((sm_count() * 6 + cblocks - 1) / cblocks);
-  chunks = chunks < 1 ? 1 : chunks;
-  int per = (L + chunks - 1) / chunks;
-  if (per < 4 * W) per = 4 * W;
-  if (per > L) per = L;
-  chunks = (L + per - 1) / per;
+  const DaySplit sp = split_days(L, cblocks, 6, 4 * W, false);
   const size_t smem = ((size_t)(W - 1) * (KA + 1) + (size_t)W * N) * kThreads * 4;
   if (smem > 227 * 1024) {
     set_error("bootstrap: %d base years x window %d need %zu bytes of shared memory per block", N, W, smem);
     return XC_ERR_UNSUPPORTED;
   }
-  dim3 grid((unsigned)cblocks, (unsigned)chunks, 1);
+  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
   return dispatch_op(op, [&](auto OPC) -> int32_t {
     constexpr int OP = decltype(OPC)::value;
     if (smem > 48 * 1024) {
@@ -708,8 +684,8 @@ int32_t launch_bootstrap(int32_t op, const float* x, int64_t C, int64_t ldx, int
                                            (int)smem);
       if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(bootstrap_kernel)");
     }
-    bootstrap_kernel<KA, KB, OP><<<grid, kThreads, smem, st>>>(x, C, ldx, base_start, N, L, W, spec, step_period, per,
-                                                               counts);
+    bootstrap_kernel<KA, KB, OP><<<grid, kThreads, smem, st>>>(x, C, ldx, base_start, N, L, W, spec, step_period,
+                                                               sp.per, counts);
     return launch_status("bootstrap_kernel");
   });
 }

@@ -111,4 +111,20 @@ inline int sm_count() {
   return n;
 }
 
+// Day split of the day-of-year kernels: blockIdx.y walks `chunks` chunks of `per` consecutive days.  Enough
+// chunks that the cblocks cell blocks give ctas_per_sm CTAs per SM, but at least min_per days per chunk (each
+// chunk pays a halo of extra days), rounded up to whole pairs of days when `pairs`.
+struct DaySplit {
+  int chunks, per;
+};
+inline DaySplit split_days(int nd, int64_t cblocks, int ctas_per_sm, int min_per, bool pairs) {
+  int chunks = (int)((sm_count() * ctas_per_sm + cblocks - 1) / cblocks);
+  if (chunks < 1) chunks = 1;
+  int per = (nd + chunks - 1) / chunks;
+  if (per < min_per) per = min_per;
+  if (pairs) per = (per + 1) & ~1;
+  if (per > nd) per = nd;
+  return {(nd + per - 1) / per, per};
+}
+
 }  // namespace xc

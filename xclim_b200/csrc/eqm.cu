@@ -22,15 +22,9 @@
 namespace xc {
 namespace {
 
-#ifndef XC_EQM_THREADS
-#define XC_EQM_THREADS 256
-#endif
-#ifndef XC_EQM_CAP
-#define XC_EQM_CAP 128
-#endif
-constexpr int kSortThreads = XC_EQM_THREADS;
+constexpr int kSortThreads = 256;
 constexpr int kBins = 1024;      // histogram bins over [min, max] of the series
-constexpr int kCap = XC_EQM_CAP; // candidates kept per needed bin
+constexpr int kCap = 128;        // candidates kept per needed bin
 constexpr int kMaxTargets = 128; // order statistics per series (2 per quantile)
 
 // Block-wide bitonic sort of keys[0..NPAD) ascending (fallback path).

@@ -34,7 +34,6 @@ namespace xc {
 namespace {
 
 constexpr int kThreads = 128;
-#define XC_NEG_INF (__int_as_float(0xff800000))
 
 __device__ __forceinline__ void store_vec4(int32_t* dst, const int32_t (&v)[4]) {
   *reinterpret_cast<int4*>(dst) = make_int4(v[0], v[1], v[2], v[3]);
@@ -46,16 +45,6 @@ __device__ __forceinline__ float prep(float v, bool top, int& n) {
   n += ok ? 1 : 0;
   v = top ? v : -v;
   return ok ? v : XC_NEG_INF;
-}
-
-template <int K>
-__device__ __forceinline__ void insert_desc(float (&lst)[K], float v) {
-#pragma unroll
-  for (int k = 0; k < K; ++k) {
-    const float hi = fmaxf(lst[k], v);
-    v = fminf(lst[k], v);
-    lst[k] = hi;
-  }
 }
 
 // Largest non-NaN value of the sample of day d, for the NaN-interpolation fallback (lerp_is_nan).
@@ -219,40 +208,23 @@ percentile_doy_select_kernel(const float* __restrict__ x, int64_t T, int64_t C, 
   }
 }
 
-#ifndef XC_PCTL_VARIANT
-#define XC_PCTL_VARIANT 0
-#endif
-#ifndef XC_PCTL_ADDR      // 0: running 64-bit pointer (2 ALU-pipe adds per load); 1: one IMAD.WIDE (FMA pipe)
-#define XC_PCTL_ADDR (XC_PCTL_VARIANT == 1 ? 1 : 0)
-#endif
-#ifndef XC_PCTL_STAGE     // 1: cp.async staging of the next day's rows in the window-5 paired kernel
-#define XC_PCTL_STAGE 1      // (an L2 prefetch of those rows was slower)
-#endif
-#ifndef XC_PCTL_PROBE     // NaN probe: 0 = compare chain (ALU pipe); 1 = FMA chain; 2 = FADD tree + 1 compare per 4
-#define XC_PCTL_PROBE (XC_PCTL_VARIANT == 1 ? 1 : 0)
-#endif
-
-// NV rows p0 + k*ystride -> v[0..NV)
+// NV rows p0 + k*ystride -> v[0..NV), through a running 64-bit pointer (two ALU-pipe adds per load)
 template <int K, int NV>
 __device__ __forceinline__ void fetch_rows(const char* p0, uint64_t ystride, float (&v)[K]) {
-#if XC_PCTL_ADDR == 1
-  const uint32_t ys32 = (uint32_t)ystride;
-#pragma unroll
-  for (int k = 0; k < NV; ++k)
-    v[k] = ld_stream(reinterpret_cast<const float*>(p0 + (uint64_t)((uint32_t)k) * (uint64_t)ys32));
-#else
   const char* pp = p0;
 #pragma unroll
   for (int k = 0; k < NV; ++k) {
     v[k] = ld_stream(reinterpret_cast<const float*>(pp));
     pp += ystride;
   }
-#endif
 }
 
 // v[0..NV) raw values -> negated for a bottom-side quantile, pads -inf, NaN -> -inf (never selected;
 // nv counts the valid ones), sorted descending.
-template <int K, int NV>
+// NaN handling stays off the fast path: only a lane that may hold a NaN looks at each value.  The probe
+// is a compare chain (min/max pipe), or with FADD_PROBE an FADD tree on the FMA pipe, which is NaN iff
+// a NaN (or +inf with -inf) is among the values and keeps the min/max pipe for the networks.
+template <int K, int NV, bool FADD_PROBE = false>
 __device__ __forceinline__ void finish_chunk(bool top, float (&v)[K], int& nv) {
 #pragma unroll
   for (int k = NV; k < K; ++k) v[k] = XC_NEG_INF;
@@ -260,29 +232,17 @@ __device__ __forceinline__ void finish_chunk(bool top, float (&v)[K], int& nv) {
 #pragma unroll
     for (int k = 0; k < NV; ++k) v[k] = -v[k];
   }
-  // NaN handling off the fast path: only a lane that may hold a NaN looks at each value
-#if XC_PCTL_PROBE == 1
-  float probe = 0.f;
-#pragma unroll
-  for (int k = 0; k < NV; ++k) probe = __fmaf_rn(v[k], 0.f, probe);
-  const bool suspicious = (probe != probe);
-#elif XC_PCTL_PROBE == 2
-  // sums of four on the FMA pipe: NaN iff a NaN (or +inf and -inf) is among them
   bool suspicious = false;
+  if constexpr (FADD_PROBE) {
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-  for (int k = 0; k < NV; k += 4) {
-    float a = v[k];
-    if (k + 1 < NV) a = __fadd_rn(a, v[k + 1]);
-    float b = (k + 2 < NV) ? v[k + 2] : 0.f;
-    if (k + 3 < NV) b = __fadd_rn(b, v[k + 3]);
-    const float q = __fadd_rn(a, b);
-    suspicious = suspicious || (q != q);
+    for (int k = 0; k < NV; ++k) acc[k & 3] = __fadd_rn(acc[k & 3], v[k]);
+    const float q = __fadd_rn(__fadd_rn(acc[0], acc[1]), __fadd_rn(acc[2], acc[3]));
+    suspicious = (q != q);
+  } else {
+#pragma unroll
+    for (int k = 0; k < NV; ++k) suspicious = suspicious || (v[k] != v[k]);
   }
-#else
-  bool suspicious = false;
-#pragma unroll
-  for (int k = 0; k < NV; ++k) suspicious = suspicious || (v[k] != v[k]);
-#endif
   nv = NV;
   if (suspicious) {
 #pragma unroll
@@ -542,9 +502,6 @@ __device__ __forceinline__ float fold_thr(double t) {
 }
 
 
-#ifndef XC_PCTL_PAIR_MINBLOCKS   // with the staging buffer 4 CTAs fit an SM (51 KB each)
-#define XC_PCTL_PAIR_MINBLOCKS 4
-#endif
 // (A day-by-day window-5 kernel with the fused per-year count of the same series -- tx90p sub-case 3a in one
 // pass -- was slower than the two-kernel path and was removed.)
 // Window 5, days handled in PAIRS.  With B(d) = Y(d-2..d+1) = A(d-1) U A(d+1) the windows of two
@@ -556,9 +513,10 @@ __device__ __forceinline__ float fold_thr(double t) {
 // copy of the day-list sort and of the final merge: two inlined copies overflow the 32 KB
 // instruction cache and cost more than the saved merges.
 // Shared memory per lane: A(d-1), the two most recent odd-position day lists Y(d-3), Y(d-1), and
-// the even-position list Y(d) waiting for its partner.
+// the even-position list Y(d) waiting for its partner; with K == 16 in uniform mode also the staging
+// column of the next day's rows (an L2 prefetch of those rows was slower), and 4 CTAs fit an SM (51 KB each).
 template <int K, bool TABLE>
-__global__ void __launch_bounds__(kThreads, XC_PCTL_PAIR_MINBLOCKS)
+__global__ void __launch_bounds__(kThreads, 4)
 percentile_doy_w5p_kernel(const float* __restrict__ x, int32_t T, int64_t C, int64_t ldx, int32_t L, int32_t N,
                           QuantSpec spec, int32_t doys_per_chunk, double* __restrict__ out,
                           const int32_t* __restrict__ pos, int32_t n_doy, int32_t d_begin, int32_t d_end) {
@@ -584,12 +542,8 @@ percentile_doy_w5p_kernel(const float* __restrict__ x, int32_t T, int64_t C, int
   int nnew, nB = 0;
 #pragma unroll
   for (int k = 0; k < K; ++k) t[k] = 0.f;
-#if XC_PCTL_STAGE
   Stager stager{reinterpret_cast<float*>(sn + 4 * kThreads) + lane, kNoDay, false};
   Stager* sg = (K == 16 && !TABLE) ? &stager : nullptr;
-#else
-  Stager* sg = nullptr;
-#endif
   // The four warm-up iterations day = p0-4 .. p0-1 run the steady-state code without emitting:
   // they leave Y(p0-2), Y(p0) in the two odd slots, A(p0) = Y(p0-1) U Y(p0) in sA and Y(p0+1) in sE
   // (what they compute from the not-yet-written lists is overwritten before it is used).  No
@@ -704,50 +658,11 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
       : "memory");
 }
 
-#ifndef XC_PCTL_TMA_MINBLOCKS
-#define XC_PCTL_TMA_MINBLOCKS 3
-#endif
-#ifndef XC_PCTL_TMA_PROBE      // 0: compare chain (min/max pipe), 2: FADD tree (FMA pipe)
-#define XC_PCTL_TMA_PROBE 2
-#endif
 constexpr int kTmaCells = kThreads;                 // cells per CTA = consumer threads
 constexpr int kTmaThreads = kThreads + 32;          // + one producer warp
 
-// values of one chunk -> descending sorted list (NaN -> -inf, counted out), cf. finish_chunk
-template <int K, int NV>
-__device__ __forceinline__ void finish_chunk_t(bool top, float (&v)[K], int& nv) {
-#pragma unroll
-  for (int k = NV; k < K; ++k) v[k] = XC_NEG_INF;
-  if (!top) {
-#pragma unroll
-    for (int k = 0; k < NV; ++k) v[k] = -v[k];
-  }
-#if XC_PCTL_TMA_PROBE == 2
-  float acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-  for (int k = 0; k < NV; ++k) acc[k & 3] = __fadd_rn(acc[k & 3], v[k]);
-  const float q = __fadd_rn(__fadd_rn(acc[0], acc[1]), __fadd_rn(acc[2], acc[3]));
-  const bool suspicious = (q != q);
-#else
-  bool suspicious = false;
-#pragma unroll
-  for (int k = 0; k < NV; ++k) suspicious = suspicious || (v[k] != v[k]);
-#endif
-  nv = NV;
-  if (suspicious) {
-#pragma unroll
-    for (int k = 0; k < NV; ++k) {
-      const bool bad = (v[k] != v[k]);
-      nv -= bad ? 1 : 0;
-      v[k] = bad ? XC_NEG_INF : v[k];
-    }
-  }
-  if constexpr (NV == K) sort_desc<K>(v);
-  else sort_desc_first<K, NV>(v);
-}
-
 template <int N2>   // years = 16 + N2, N2 in {14, 15, 16}
-__global__ void __launch_bounds__(kTmaThreads, XC_PCTL_TMA_MINBLOCKS)
+__global__ void __launch_bounds__(kTmaThreads, 3)
 percentile_doy_w5t_kernel(const __grid_constant__ CUtensorMap tmap, int64_t C, int32_t L, QuantSpec spec,
                           int32_t doys_per_chunk, double* __restrict__ out, int32_t d_begin, int32_t d_end,
                           const float* __restrict__ x, int64_t ldx) {
@@ -825,8 +740,8 @@ percentile_doy_w5t_kernel(const __grid_constant__ CUtensorMap tmap, int64_t C, i
       __syncwarp();
       if ((lane & 31) == 0) mbar_arrive(&empty[st]);    // this warp has read the tile
       int n1, n2;
-      finish_chunk_t<K, K>(top, ynew, n1);
-      finish_chunk_t<K, N2>(top, v2, n2);
+      finish_chunk<K, K, true>(top, ynew, n1);
+      finish_chunk<K, N2, true>(top, v2, n2);
       nnew = n1 + n2;
       merge_top_desc<K>(ynew, v2);
     }
@@ -1107,23 +1022,25 @@ doy_count_years_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int6
   }
 }
 
-template <int K>
-int32_t launch_generic(const float* x, int64_t T, int64_t C, int64_t ldx, const int32_t* pos, int32_t n_doy,
+// generic kernel with the shortest list that holds `need` (<= 64) order statistics
+int32_t launch_generic(int need, const float* x, int64_t T, int64_t C, int64_t ldx, const int32_t* pos, int32_t n_doy,
                        int32_t n_years, int32_t h, const QuantSpec& spec, double* out, cudaStream_t st,
                        int d_begin = 0, int d_end = -1, const int32_t* vrow = nullptr) {
   if (d_end < 0) d_end = n_doy;
   const int nd = d_end - d_begin;
   if (nd <= 0) return XC_OK;
   const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  // enough chunks to fill the machine when the grid is narrow
-  int chunks = (int)((sm_count() * 8 + cblocks - 1) / cblocks);
-  chunks = chunks < 1 ? 1 : (chunks > nd ? nd : chunks);
-  const int per = (nd + chunks - 1) / chunks;
-  chunks = (nd + per - 1) / per;
-  dim3 grid((unsigned)cblocks, (unsigned)chunks, 1);
-  percentile_doy_generic_kernel<K><<<grid, kThreads, 0, st>>>(x, T, C, ldx, pos, n_doy, n_years, h, spec, per, out,
-                                                              d_begin, d_end, vrow);
-  return launch_status("percentile_doy_generic_kernel");
+  const DaySplit sp = split_days(nd, cblocks, 8, 1, false);
+  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
+  auto go = [&](auto kern) -> int32_t {
+    kern<<<grid, kThreads, 0, st>>>(x, T, C, ldx, pos, n_doy, n_years, h, spec, sp.per, out, d_begin, d_end, vrow);
+    return launch_status("percentile_doy_generic_kernel");
+  };
+  if (need <= 4) return go(percentile_doy_generic_kernel<4>);
+  if (need <= 8) return go(percentile_doy_generic_kernel<8>);
+  if (need <= 16) return go(percentile_doy_generic_kernel<16>);
+  if (need <= 32) return go(percentile_doy_generic_kernel<32>);
+  return go(percentile_doy_generic_kernel<64>);
 }
 
 // pos == nullptr: uniform years (days [0, L)); else table mode on the interior days [d_begin, d_end)
@@ -1135,12 +1052,8 @@ int32_t launch_uniform(const float* x, int64_t T, int64_t C, int64_t ldx, int32_
   const int nd = d_end - d_begin;
   if (nd <= 0) return XC_OK;
   const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  int chunks = (int)((sm_count() * 12 + cblocks - 1) / cblocks);
-  chunks = chunks < 1 ? 1 : chunks;
-  int per = (nd + chunks - 1) / chunks;
-  if (per < 8 * W) per = 8 * W;  // keep the halo overhead (W-1 extra day lists per chunk) small
-  if (per > nd) per = nd;
-  chunks = (nd + per - 1) / per;
+  // at least 8 W days per chunk keeps the halo overhead (W-1 extra day lists per chunk) small
+  const DaySplit sp = split_days(nd, cblocks, 12, 8 * W, false);
   const size_t smem = (size_t)(W - 1) * (K + 1) * kThreads * 4;
   if (smem > 48 * 1024) {
     cudaError_t e = pos ? cudaFuncSetAttribute(percentile_doy_uniform_kernel<K, true>,
@@ -1149,12 +1062,12 @@ int32_t launch_uniform(const float* x, int64_t T, int64_t C, int64_t ldx, int32_
                                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(percentile_doy_uniform_kernel)");
   }
-  dim3 grid((unsigned)cblocks, (unsigned)chunks, 1);
+  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
   if (pos)
-    percentile_doy_uniform_kernel<K, true><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, W, spec, per,
+    percentile_doy_uniform_kernel<K, true><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, W, spec, sp.per,
                                                                          out, pos, n_doy, d_begin, d_end);
   else
-    percentile_doy_uniform_kernel<K, false><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, W, spec, per,
+    percentile_doy_uniform_kernel<K, false><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, W, spec, sp.per,
                                                                           out, pos, n_doy, d_begin, d_end);
   return launch_status("percentile_doy_uniform_kernel");
 }
@@ -1167,16 +1080,10 @@ int32_t launch_w5(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t L, 
   const int nd = d_end - d_begin;
   if (nd <= 0) return XC_OK;
   const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  int chunks = (int)((sm_count() * 16 + cblocks - 1) / cblocks);
-  chunks = chunks < 1 ? 1 : chunks;
-  int per = (nd + chunks - 1) / chunks;
-  if (per < 40) per = 40;  // 4 extra day lists per chunk
-  per = (per + 1) & ~1;    // whole pairs of days
-  if (per > nd) per = nd;
-  chunks = (nd + per - 1) / per;
+  const DaySplit sp = split_days(nd, cblocks, 16, 40, true);   // 4 extra day lists per chunk, whole pairs of days
   // 4 lists + 4 counts per lane, plus the 32-row staging column of the cp.async prefetch
-  const size_t smem = (size_t)4 * (K + 1) * kThreads * 4 + (XC_PCTL_STAGE && K == 16 && !pos ? (size_t)32 * kThreads * 4 : 0);
-  dim3 grid((unsigned)cblocks, (unsigned)chunks, 1);
+  const size_t smem = (size_t)4 * (K + 1) * kThreads * 4 + (K == 16 && !pos ? (size_t)32 * kThreads * 4 : 0);
+  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
   if (smem > 48 * 1024) {
     cudaError_t e = pos ? cudaFuncSetAttribute(percentile_doy_w5p_kernel<K, true>,
                                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
@@ -1185,12 +1092,25 @@ int32_t launch_w5(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t L, 
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(percentile_doy_w5p_kernel)");
   }
   if (pos)
-    percentile_doy_w5p_kernel<K, true><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, spec, per, out, pos,
-                                                                     n_doy, d_begin, d_end);
+    percentile_doy_w5p_kernel<K, true><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, spec, sp.per, out,
+                                                                     pos, n_doy, d_begin, d_end);
   else
-    percentile_doy_w5p_kernel<K, false><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, spec, per, out,
+    percentile_doy_w5p_kernel<K, false><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, spec, sp.per, out,
                                                                       pos, n_doy, d_begin, d_end);
   return launch_status("percentile_doy_w5p_kernel");
+}
+
+// Day-list kernel for `need` (<= 32) order statistics and window `W`: the paired kernel for window 5 and
+// need <= 16, else the ring kernel.  pos == nullptr: uniform years; else table mode on [d_begin, d_end).
+int32_t launch_day_lists(int need, int32_t W, const float* x, int64_t T, int64_t C, int64_t ldx, int32_t L, int32_t N,
+                         const QuantSpec& spec, double* out, cudaStream_t st, const int32_t* pos = nullptr,
+                         int n_doy = 0, int d_begin = 0, int d_end = -1) {
+  if (W == 5 && need <= 16)
+    return need <= 8 ? launch_w5<8>(x, T, C, ldx, L, N, spec, out, st, pos, n_doy, d_begin, d_end)
+                     : launch_w5<16>(x, T, C, ldx, L, N, spec, out, st, pos, n_doy, d_begin, d_end);
+  if (need <= 8) return launch_uniform<8>(x, T, C, ldx, L, N, W, spec, out, st, pos, n_doy, d_begin, d_end);
+  if (need <= 16) return launch_uniform<16>(x, T, C, ldx, L, N, W, spec, out, st, pos, n_doy, d_begin, d_end);
+  return launch_uniform<32>(x, T, C, ldx, L, N, W, spec, out, st, pos, n_doy, d_begin, d_end);
 }
 
 
@@ -1228,21 +1148,14 @@ int32_t launch_w5_tma(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NAN_REQUEST_ZERO_FMA);
   if (r != CUDA_SUCCESS) return 1;
-  const int nd = L;
   const int64_t cblocks = (C + kTmaCells - 1) / kTmaCells;
-  int chunks = (int)((sm_count() * 12 + cblocks - 1) / cblocks);
-  chunks = chunks < 1 ? 1 : chunks;
-  int per = (nd + chunks - 1) / chunks;
-  if (per < 40) per = 40;  // 4 extra day lists per chunk
-  per = (per + 1) & ~1;    // whole pairs of days
-  if (per > nd) per = nd;
-  chunks = (nd + per - 1) / per;
+  const DaySplit sp = split_days(L, cblocks, 12, 40, true);   // 4 extra day lists per chunk, whole pairs of days
   const size_t smem = (size_t)2 * N * kTmaCells * 4 + (size_t)4 * (16 + 1) * kThreads * 4 + 64;
-  dim3 grid((unsigned)cblocks, (unsigned)chunks, 1);
+  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
   auto go = [&](auto kern) -> int32_t {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(percentile_doy_w5t_kernel)");
-    kern<<<grid, kTmaThreads, smem, st>>>(map, C, L, spec, per, out, 0, L, x, ldx);
+    kern<<<grid, kTmaThreads, smem, st>>>(map, C, L, spec, sp.per, out, 0, L, x, ldx);
     return launch_status("percentile_doy_w5t_kernel");
   };
   if (N == 30) return go(percentile_doy_w5t_kernel<14>);
@@ -1262,6 +1175,19 @@ extern "C" int64_t xc_percentile_doy_workspace_bytes(int64_t T, int64_t C, int32
   return 2 * (int64_t)n_doy * (int64_t)n_years * 4 + T * 4 + 256;
 }
 
+// (year, doy) -> step table: pos[y * n_doy + d - 1] = the step of day-of-year d of year y, -1 where there is
+// none.  Returns the first step whose indexes are out of range, or -1.
+static int64_t build_pos_table(int64_t T, const int16_t* doy_index_host, const int16_t* year_index_host,
+                               int32_t n_doy, int32_t n_years, std::vector<int32_t>& pos) {
+  pos.assign((size_t)n_doy * n_years, -1);
+  for (int64_t t = 0; t < T; ++t) {
+    const int d = doy_index_host[t], y = year_index_host[t];
+    if (d < 1 || d > n_doy || y < 0 || y >= n_years) return t;
+    pos[(size_t)y * n_doy + (d - 1)] = (int32_t)t;
+  }
+  return -1;
+}
+
 static int32_t percentile_doy_impl(const float* x, int64_t T, int64_t C, int64_t ldx,
                                    const int16_t* doy_index_host, const int16_t* year_index_host,
                                    int32_t n_doy, int32_t n_years, int32_t window,
@@ -1279,20 +1205,20 @@ static int32_t percentile_doy_impl(const float* x, int64_t T, int64_t C, int64_t
   const int h = window / 2;
   cudaStream_t st = (cudaStream_t)stream;
 
-  // (year, doy) -> row table, and detection of the uniform-year fast path
-  std::vector<int32_t> pos((size_t)n_doy * n_years, -1);
-  bool uniform = (T == (int64_t)n_doy * n_years);
-  for (int64_t t = 0; t < T; ++t) {
-    const int d = doy_index_host[t], y = year_index_host[t];
-    XC_REQUIRE(d >= 1 && d <= n_doy && y >= 0 && y < n_years, "doy/year index out of range at step %lld", (long long)t);
-    pos[(size_t)y * n_doy + (d - 1)] = (int32_t)t;
-    if (uniform && (d - 1 != (int)(t % n_doy) || y != (int)(t / n_doy))) uniform = false;
-  }
+  std::vector<int32_t> pos;
+  const int64_t bad = build_pos_table(T, doy_index_host, year_index_host, n_doy, n_years, pos);
+  XC_REQUIRE(bad < 0, "doy/year index out of range at step %lld", (long long)bad);
+  // uniform-year fast path: step t is day t % n_doy of year t / n_doy
+  bool uniform = !vrow_host && T == (int64_t)pos.size();
+  for (size_t k = 0; uniform && k < pos.size(); ++k) uniform = (pos[k] == (int32_t)k);
+
   int32_t* pos_d = nullptr;      // (year, doy) -> step
   int32_t* posrow_d = nullptr;   // (year, doy) -> row holding that step's value (== pos_d without vrow)
   int32_t* vrow_d = nullptr;     // step -> row
-  if (vrow_host) uniform = false;
-  if (!uniform) {
+  // The tables go to the workspace when the first kernel that reads them is launched, so a uniform
+  // calendar served by the day-list kernels needs no workspace.
+  auto upload_tables = [&]() -> int32_t {
+    if (pos_d) return XC_OK;
     const int64_t nb = (int64_t)pos.size() * 4;
     const int64_t need = vrow_host ? 2 * nb + T * 4 : nb;
     XC_REQUIRE(workspace != nullptr && workspace_bytes >= need, "workspace too small: need %lld bytes", (long long)need);
@@ -1312,6 +1238,12 @@ static int32_t percentile_doy_impl(const float* x, int64_t T, int64_t C, int64_t
     }
     // the tables live on this stack frame: make sure the copies have been issued from pageable memory
     XC_CHECK_CUDA(cudaStreamSynchronize(st));
+    return XC_OK;
+  };
+  // every kernel reads them when the years differ: check the workspace (and vrow) before anything else
+  if (!uniform) {
+    const int32_t e = upload_tables();
+    if (e) return e;
   }
 
   // interior days whose windows never leave the year: [h, L_int - h) with L_int the shortest full year
@@ -1335,27 +1267,17 @@ static int32_t percentile_doy_impl(const float* x, int64_t T, int64_t C, int64_t
                   nmax);
         return XC_ERR_UNSUPPORTED;
       }
-      if (pos_d == nullptr) {
-        const int64_t nbytes = (int64_t)pos.size() * 4;
-        XC_REQUIRE(workspace != nullptr && workspace_bytes >= nbytes, "workspace too small: need %lld bytes",
-                   (long long)nbytes);
-        pos_d = (int32_t*)workspace;
-        posrow_d = pos_d;
-        XC_CHECK_CUDA(cudaMemcpyAsync(pos_d, pos.data(), (size_t)nbytes, cudaMemcpyHostToDevice, st));
-        XC_CHECK_CUDA(cudaStreamSynchronize(st));
-      }
+      const int32_t eu = upload_tables();
+      if (eu) return eu;
       const size_t smem = (size_t)nmax * kSelThreads * 4;
       if (smem > 48 * 1024)
         XC_CHECK_CUDA(cudaFuncSetAttribute(percentile_doy_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)smem));
       const int64_t cblocks = (C + kSelThreads - 1) / kSelThreads;
-      int chunks = (int)((sm_count() * 8 + cblocks - 1) / cblocks);
-      chunks = chunks < 1 ? 1 : (chunks > n_doy ? n_doy : chunks);
-      const int per_chunk = (n_doy + chunks - 1) / chunks;
-      chunks = (n_doy + per_chunk - 1) / per_chunk;
-      dim3 grid((unsigned)cblocks, (unsigned)chunks, 1);
+      const DaySplit sp = split_days(n_doy, cblocks, 8, 1, false);
+      dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
       percentile_doy_select_kernel<<<grid, kSelThreads, smem, st>>>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec,
-                                                                    per_chunk, o, vrow_d);
+                                                                    sp.per, o, vrow_d);
       const int32_t es = launch_status("percentile_doy_select_kernel");
       if (es) return es;
       continue;
@@ -1365,26 +1287,13 @@ static int32_t percentile_doy_impl(const float* x, int64_t T, int64_t C, int64_t
     const bool fast_ok = window >= 3 && need <= 32 && smem_need <= 200 * 1024 && (L_int - 2 * h) >= 8;
     int32_t e = XC_OK;
     if (uniform && fast_ok) {
-      if (window == 5 && need <= 16) {
-        e = 1;
-        if (need > 8 && !getenv("XCLIM_B200_NO_TMA")) e = launch_w5_tma(x, T, C, ldx, n_doy, n_years, spec, o, st);
-        if (e == 1)
-          e = need <= 8 ? launch_w5<8>(x, T, C, ldx, n_doy, n_years, spec, o, st)
-                        : launch_w5<16>(x, T, C, ldx, n_doy, n_years, spec, o, st);
-      } else
-        e = need <= 8    ? launch_uniform<8>(x, T, C, ldx, n_doy, n_years, window, spec, o, st)
-            : need <= 16 ? launch_uniform<16>(x, T, C, ldx, n_doy, n_years, window, spec, o, st)
-                         : launch_uniform<32>(x, T, C, ldx, n_doy, n_years, window, spec, o, st);
+      e = 1;
+      if (window == 5 && need > 8 && need <= 16 && !getenv("XCLIM_B200_NO_TMA"))
+        e = launch_w5_tma(x, T, C, ldx, n_doy, n_years, spec, o, st);
+      if (e == 1) e = launch_day_lists(need, window, x, T, C, ldx, n_doy, n_years, spec, o, st);
     } else {
-      if (pos_d == nullptr) {  // uniform calendar without a fast instantiation: the table is still needed
-        const int64_t nbytes = (int64_t)pos.size() * 4;
-        XC_REQUIRE(workspace != nullptr && workspace_bytes >= nbytes, "workspace too small: need %lld bytes",
-                   (long long)nbytes);
-        pos_d = (int32_t*)workspace;
-        posrow_d = pos_d;
-        XC_CHECK_CUDA(cudaMemcpyAsync(pos_d, pos.data(), (size_t)nbytes, cudaMemcpyHostToDevice, st));
-        XC_CHECK_CUDA(cudaStreamSynchronize(st));
-      }
+      e = upload_tables();  // a uniform calendar without a fast instantiation still needs the table
+      if (e) return e;
       // Days whose samples decompose into per-day lists: the window must stay inside the year
       // ([h, L_int - h)) and no window centre may fall outside the series (the h days before the first
       // step's day-of-year and after the last step's: their neighbours exist but their centres do not).
@@ -1401,22 +1310,10 @@ static int32_t percentile_doy_impl(const float* x, int64_t T, int64_t C, int64_t
         int b = a;
         const bool fast = fast_day[a] != 0;
         while (b < n_doy && (fast_day[b] != 0) == fast) ++b;
-        if (fast && (b - a) >= 8) {
-          if (window == 5 && need <= 16)
-            e = need <= 8 ? launch_w5<8>(x, T, C, ldx, n_doy, n_years, spec, o, st, posrow_d, n_doy, a, b)
-                          : launch_w5<16>(x, T, C, ldx, n_doy, n_years, spec, o, st, posrow_d, n_doy, a, b);
-          else
-            e = need <= 8    ? launch_uniform<8>(x, T, C, ldx, n_doy, n_years, window, spec, o, st, posrow_d, n_doy, a, b)
-                : need <= 16 ? launch_uniform<16>(x, T, C, ldx, n_doy, n_years, window, spec, o, st, posrow_d, n_doy, a, b)
-                             : launch_uniform<32>(x, T, C, ldx, n_doy, n_years, window, spec, o, st, posrow_d, n_doy,
-                                                  a, b);
-        } else {
-          if (need <= 4) e = launch_generic<4>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec, o, st, a, b, vrow_d);
-          else if (need <= 8) e = launch_generic<8>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec, o, st, a, b, vrow_d);
-          else if (need <= 16) e = launch_generic<16>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec, o, st, a, b, vrow_d);
-          else if (need <= 32) e = launch_generic<32>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec, o, st, a, b, vrow_d);
-          else e = launch_generic<64>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec, o, st, a, b, vrow_d);
-        }
+        if (fast && (b - a) >= 8)
+          e = launch_day_lists(need, window, x, T, C, ldx, n_doy, n_years, spec, o, st, posrow_d, n_doy, a, b);
+        else
+          e = launch_generic(need, x, T, C, ldx, pos_d, n_doy, n_years, h, spec, o, st, a, b, vrow_d);
         if (e) return e;
         a = b;
       }
@@ -1454,12 +1351,9 @@ extern "C" int32_t xc_percentile_doy_generic_f32(const float* x, int64_t T, int6
                                                  int64_t workspace_bytes, void* stream) {
   XC_REQUIRE(x && doy_index_host && year_index_host && out && workspace, "null pointer argument");
   XC_REQUIRE(window >= 1 && window % 2 == 1, "window must be odd");
-  std::vector<int32_t> pos((size_t)n_doy * n_years, -1);
-  for (int64_t t = 0; t < T; ++t) {
-    const int d = doy_index_host[t], y = year_index_host[t];
-    XC_REQUIRE(d >= 1 && d <= n_doy && y >= 0 && y < n_years, "doy/year index out of range");
-    pos[(size_t)y * n_doy + (d - 1)] = (int32_t)t;
-  }
+  std::vector<int32_t> pos;
+  XC_REQUIRE(build_pos_table(T, doy_index_host, year_index_host, n_doy, n_years, pos) < 0,
+             "doy/year index out of range");
   const int64_t need_b = (int64_t)pos.size() * 4;
   XC_REQUIRE(workspace_bytes >= need_b, "workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1471,13 +1365,7 @@ extern "C" int32_t xc_percentile_doy_generic_f32(const float* x, int64_t T, int6
     set_error("percentile needs %d order statistics; at most 64 are kept", need);
     return XC_ERR_UNSUPPORTED;
   }
-  const int32_t* pos_d = (const int32_t*)workspace;
-  const int h = window / 2;
-  if (need <= 4) return launch_generic<4>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec, out, st);
-  if (need <= 8) return launch_generic<8>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec, out, st);
-  if (need <= 16) return launch_generic<16>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec, out, st);
-  if (need <= 32) return launch_generic<32>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec, out, st);
-  return launch_generic<64>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec, out, st);
+  return launch_generic(need, x, T, C, ldx, (const int32_t*)workspace, n_doy, n_years, window / 2, spec, out, st);
 }
 
 extern "C" int32_t xc_doy_interp_f64(const double* table, int32_t n_src, int64_t C, int32_t doy_min,

@@ -12,6 +12,8 @@
 
 namespace xc {
 
+#define XC_NEG_INF (__int_as_float(0xff800000))
+
 struct QuantSpec {
   double q;      // quantile in [0, 1]
   double c;      // alpha + q*(1 - alpha - beta)   (evaluated on the host with the same operations)
@@ -43,6 +45,17 @@ inline int plan_quantile(double per, double alpha, double beta, int n_max, Quant
   if (top_ok && (ktop <= kbot || !bot_ok)) { spec->top = 1; return ktop; }
   if (bot_ok) { spec->top = 0; return kbot; }
   return -1;  // alpha/beta outside [0, 1] with a mid quantile: not supported
+}
+
+// inserts v into the descending list lst, dropping its smallest entry (2K min/max)
+template <int K>
+__device__ __forceinline__ void insert_desc(float (&lst)[K], float v) {
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    const float hi = fmaxf(lst[k], v);
+    v = fminf(lst[k], v);
+    lst[k] = hi;
+  }
 }
 
 template <int K>
