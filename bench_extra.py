@@ -201,6 +201,22 @@ def main():
             haf, hhq = O.eqm_train(host["tas"], host["hist"], 20, "+")
         report("eqm_adjust linear (sim -> scen)", ms, 2 * T * C * 4 + 2 * 20 * C * 4,
                cpu=lambda: O.eqm_adjust(host["hist"], haf, hhq, "+", "linear"))
+    if want("qdm"):
+        from xclim_b200.sdba import equally_spaced_nodes
+        hist = af = hq = None      # the EQM section's buffers: sim, scen and sim_q need the room
+        hist = device.synth(T, C, kind=1, seed=5, cells_per_lat=X, n_lat_global=a.lat)
+        af, _ = device.eqm_train(tas, hist, 20, 0)
+        nodes = equally_spaced_nodes(20).astype(np.float32)
+        if a.cpu:
+            from oracle import qdm_oracle as QO
+            host["hist"] = hist[:, :S].cpu().numpy()
+            qaf = af[:, :S].cpu().numpy()
+        for with_q in (False, True):
+            ms = timeit(lambda: device.qdm_adjust(hist, af, nodes, 0, 1, want_sim_q=with_q), a.steps)
+            report("qdm_adjust linear nq=20 (sim -> scen" + (", sim_q float64)" if with_q else ")"), ms,
+                   2 * T * C * 4 + 20 * C * 4 + (T * C * 8 if with_q else 0),
+                   {"scratch_bytes_per_cell": 6 * T + 16},
+                   cpu=lambda: QO.qdm_adjust(host["hist"], qaf, "+", "linear"))
     if want("fwi") and a.only:      # the fire-weather kernel: opt-in (--only fwi), never part of a default run
         import time
 

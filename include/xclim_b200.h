@@ -350,6 +350,27 @@ int32_t xc_eqm_adjust_f32(const float* sim, int64_t T, int64_t C, int64_t ldx,
                           int32_t kind, int32_t interp, float* scen, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * a20 (cont.)  quantile delta mapping -- xsdba.QuantileDeltaMapping (third-party, re-exported by
+ *   sdba.py:11; its train step is EmpiricalQuantileMapping.train, i.e. xc_eqm_train_f32).
+ *   group="time", extrapolation="constant".  Per cell of sim (T, C):
+ *     sim_q = percentage rank of sim within the cell's whole series (average ranks of ties over the
+ *             n valid values, p = r / n, then (mx * (p - mn)) / (mx - mn) with mn / mx the min / max
+ *             of p; float64; NaN where sim is NaN or the cell has fewer than two distinct values);
+ *     scen  = sim (+|*) interp(sim_q; nodes -> af) in float32, af entries that are NaN dropped,
+ *             interp 0 = nearest (ties to the lower node), 1 = linear, constant end factors.
+ *   nodes: device float32[nq], the quantile nodes of af (equally_spaced_nodes(nq) as float32).
+ *   af: (nq, C) float32 with leading dimension C.  sim_q: (T, C) float64 or NULL.
+ *   workspace: device scratch; any size >= xc_qdm_adjust_workspace_bytes(T, 32) works (the cells are
+ *   processed in chunks that fit), xc_qdm_adjust_workspace_bytes(T, C) processes all cells at once.
+ *   T <= 32768 (longer series return XC_ERR_UNSUPPORTED).
+ * ------------------------------------------------------------------------------------------- */
+int64_t xc_qdm_adjust_workspace_bytes(int64_t T, int64_t C);
+int32_t xc_qdm_adjust_f32(const float* sim, int64_t T, int64_t C, int64_t ldx,
+                          const float* af, const float* nodes, int32_t nq, int32_t kind, int32_t interp,
+                          float* scen, double* sim_q, void* workspace, int64_t workspace_bytes,
+                          void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Synthetic inputs (BASELINE.json configs; SURVEY.md section 8d).  Stateless counter-based
  * generators: value(t, global_cell) depends only on (seed, t, global_cell), so a lat tile
  * generated on any rank equals the same slab of the global grid.

@@ -98,6 +98,25 @@ inline int32_t dispatch_op_nan(int32_t op, F&& f) {
   return dispatch_op(op, f);
 }
 
+// Block-wide bitonic sort of keys[0..NPAD) ascending in shared memory by NT threads (NaN-free keys): the
+// fallback sort of the EQM train and QDM rank kernels.
+template <int NPAD, int NT>
+__device__ void block_bitonic_sort(float* keys, int tid) {
+  for (int k = 2; k <= NPAD; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = tid; i < NPAD / 2; i += NT) {
+        const int a = ((i & ~(j - 1)) << 1) | (i & (j - 1));  // pair (a, a | j)
+        const int b = a | j;
+        const bool up = ((a & k) == 0);
+        const float x0 = keys[a], x1 = keys[b];
+        const bool swap = up ? (x0 > x1) : (x0 < x1);
+        if (swap) { keys[a] = x1; keys[b] = x0; }
+      }
+      __syncthreads();
+    }
+  }
+}
+
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // SMs of the current device (132 on an H100 SXM, 114 on an H100 PCIe): launchers that split a narrow grid

@@ -27,24 +27,6 @@ constexpr int kBins = 1024;      // histogram bins over [min, max] of the series
 constexpr int kCap = 128;        // candidates kept per needed bin
 constexpr int kMaxTargets = 128; // order statistics per series (2 per quantile)
 
-// Block-wide bitonic sort of keys[0..NPAD) ascending (fallback path).
-template <int NPAD>
-__device__ void block_bitonic_sort(float* keys, int tid) {
-  for (int k = 2; k <= NPAD; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = tid; i < NPAD / 2; i += kSortThreads) {
-        const int a = ((i & ~(j - 1)) << 1) | (i & (j - 1));  // pair (a, a | j)
-        const int b = a | j;
-        const bool up = ((a & k) == 0);
-        const float x0 = keys[a], x1 = keys[b];
-        const bool swap = up ? (x0 > x1) : (x0 < x1);
-        if (swap) { keys[a] = x1; keys[b] = x0; }
-      }
-      __syncthreads();
-    }
-  }
-}
-
 // One CTA = one cell.  The nq quantiles need only ~2*nq order statistics, so instead of sorting the
 // series the CTA (1) histograms it over kBins equal-width bins between its min and max (binning by a
 // monotone float expression keeps bins ordered), (2) locates the bin and the in-bin rank of every
@@ -218,7 +200,7 @@ eqm_train_kernel(const float* __restrict__ ref, const float* __restrict__ hist, 
         keys[t] = v;
       }
       __syncthreads();
-      block_bitonic_sort<NPAD>(keys, tid);
+      block_bitonic_sort<NPAD, kSortThreads>(keys, tid);
       for (int g = tid; g < ntg; g += kSortThreads) tgt_val[g] = keys[tgt_rank[g] + hist_s[tgt_bin[g]]];
       __syncthreads();
     }

@@ -343,6 +343,36 @@ def eqm_adjust(sim2d, af, hq, kind_code, interp_code):
     return scen
 
 
+#: upper bound of the QDM ranking scratch; larger grids are ranked in chunks of cells (6 T + 16 bytes per cell)
+QDM_WORKSPACE_CAP = 2 << 30
+
+
+def qdm_adjust(sim2d, af, nodes, kind_code, interp_code, want_sim_q=False, workspace_bytes=None):
+    """Quantile delta mapping adjust (xc_qdm_adjust_f32): ``scen`` (T, C) float32 and, with ``want_sim_q``, the
+    float64 percentage ranks ``sim_q`` (else None).  ``nodes``: the nq float32 quantile nodes of ``af`` (nq, C).
+    ``workspace_bytes`` (default: all cells at once, capped by QDM_WORKSPACE_CAP; the smallest workspace when that
+    does not fit) sets the ranking scratch, hence the number of cell chunks."""
+    T, C = sim2d.shape
+    nq = af.shape[0]
+    assert af.shape == (nq, C) and af.is_contiguous() and af.dtype == torch.float32
+    lib = load()
+    if workspace_bytes is None:
+        try:
+            ws = torch.empty(min(int(lib.xc_qdm_adjust_workspace_bytes(T, C)), QDM_WORKSPACE_CAP), dtype=torch.uint8,
+                             device=sim2d.device)
+        except torch.cuda.OutOfMemoryError:
+            ws = torch.empty(int(lib.xc_qdm_adjust_workspace_bytes(T, 32)), dtype=torch.uint8, device=sim2d.device)
+    else:
+        ws = torch.empty(int(workspace_bytes), dtype=torch.uint8, device=sim2d.device)
+    nodes_d = torch.as_tensor(np.asarray(nodes, dtype=np.float32)).to(sim2d.device)
+    scen = torch.empty((T, C), dtype=torch.float32, device=sim2d.device)
+    sim_q = torch.empty((T, C), dtype=torch.float64, device=sim2d.device) if want_sim_q else None
+    check(lib.xc_qdm_adjust_f32(sim2d.data_ptr(), T, C, sim2d.stride(0), af.data_ptr(), nodes_d.data_ptr(), nq,
+                                kind_code, interp_code, scen.data_ptr(), _ptr(sim_q), ws.data_ptr(), ws.numel(),
+                                current_stream_ptr()))
+    return scen, sim_q
+
+
 def period_boundary_run(x2d, poff, op_code, thr, window, last=False, cmp_f64=False):
     """Index of the first (last) run of >= window steps per period, NaN if none (run_length.py:543-740)."""
     T, C = x2d.shape

@@ -15,10 +15,15 @@ tests/test_indices.py:4116-4126) or is dropped (what its whole-array ``rle`` doe
 
 ``stream_min_bytes`` / ``stream_slab_bytes``: host-backed inputs at least this large are streamed through HBM
 in lat slabs of about ``stream_slab_bytes`` (H2D of slab k+1 overlapped with the kernels of slab k).
+
+``sdba_extra_output`` (default False): ``sdba.QuantileDeltaMapping.adjust`` returns ``{"scen": ..., "sim_q": ...}``
+(``sim_q``: the float64 percentage ranks of ``sim``) instead of ``scen`` alone, like ``xsdba.set_options(
+extra_output=True)``.
 """
 from __future__ import annotations
 
 OPTIONS = {"device_outputs": False, "rle_nan_adjacent": "count", "check_missing": "any", "missing_options": {},
+           "sdba_extra_output": False,
            # end-to-end slab streaming of host inputs (xclim_b200/streaming.py): inputs smaller than
            # stream_min_bytes are unwrapped in one piece; one slab of one input is about stream_slab_bytes
            "stream_min_bytes": 256 << 20, "stream_slab_bytes": 1 << 30, "_in_stream": False}

@@ -1,9 +1,10 @@
-"""CUDA implementation behind ``xclim.sdba.EmpiricalQuantileMapping`` (xsdba; PARITY UNPINNED).
+"""CUDA implementation behind ``xclim.sdba.EmpiricalQuantileMapping`` and ``QuantileDeltaMapping`` (xsdba;
+PARITY UNPINNED).
 
 ``xclim.sdba`` is a shim over the third-party ``xsdba`` package (sdba.py:11) whose sources are not
 part of the reference tree; the algorithm below follows its published behaviour and the reference's
 call sites (tests/test_xsdba.py:21-34, 143-150): ``EQM.train(ref, hist, nquantiles=, kind=,
-group="time")`` then ``.adjust(sim, interp=, extrapolation="constant")``.
+group="time")`` then ``.adjust(sim, interp=, extrapolation="constant")``; QDM trains the same way.
 """
 from __future__ import annotations
 
@@ -12,6 +13,7 @@ import numpy as np
 from . import device
 from .field import attrs_of, wrap_like
 from .generic import _unwrap
+from .options import OPTIONS
 
 _KINDS = {"+": 0, "*": 1}
 _INTERP = {"nearest": 0, "linear": 1}
@@ -58,7 +60,8 @@ class EmpiricalQuantileMapping:
                              attrs={"kind": self.kind, "group": "time"}, name=name)
         return {"af": wrap(self._af, "af"), "hist_q": wrap(self._hq, "hist_q")}
 
-    def adjust(self, sim, *, interp="nearest", extrapolation="constant", **kwargs):
+    def _unwrap_sim(self, sim, interp, extrapolation, kwargs):
+        """Validate the adjust options and unwrap ``sim`` to (T, C): ``(s2, other_dims, time_axis)``."""
         if interp not in _INTERP:
             raise NotImplementedError(f"interp={interp!r} is not supported (nearest, linear)")
         if extrapolation != "constant":
@@ -68,8 +71,36 @@ class EmpiricalQuantileMapping:
         s2, cell_shape, other, ta = _unwrap(sim)
         if cell_shape != self._cell_shape:
             raise ValueError("sim grid differs from the training grid")
-        scen = device.eqm_adjust(s2, self._af, self._hq, _KINDS[self.kind], _INTERP[interp])
-        vals = scen.reshape((scen.shape[0],) + cell_shape).cpu().numpy()
-        attrs = attrs_of(sim)
+        return s2, other, ta
+
+    def _wrap_series(self, sim, values, other, ta, name, attrs):
+        vals = values.reshape((values.shape[0],) + self._cell_shape).cpu().numpy()
         return wrap_like(sim, vals, ("time",) + other, time=ta if ta.coord is None else ta.coord, attrs=attrs,
-                         name="scen")
+                         name=name)
+
+    def adjust(self, sim, *, interp="nearest", extrapolation="constant", **kwargs):
+        s2, other, ta = self._unwrap_sim(sim, interp, extrapolation, kwargs)
+        scen = device.eqm_adjust(s2, self._af, self._hq, _KINDS[self.kind], _INTERP[interp])
+        return self._wrap_series(sim, scen, other, ta, "scen", attrs_of(sim))
+
+
+class QuantileDeltaMapping(EmpiricalQuantileMapping):
+    """Quantile delta mapping bias adjustment, group="time" (xsdba ``QuantileDeltaMapping``; PARITY UNPINNED).
+
+    ``train`` and ``.ds`` are EmpiricalQuantileMapping's.  ``adjust`` maps every value of ``sim`` through its own
+    percentage rank within the cell's series (``sim_q``) instead of through ``hist_q``, so that the simulated
+    change signal, trend included, is kept: ``scen = sim + af(sim_q)`` ("+") or ``sim * af(sim_q)`` ("*").  With
+    ``set_options(sdba_extra_output=True)`` it returns ``{"scen": ..., "sim_q": ...}`` (``sim_q`` in float64).
+    """
+
+    def adjust(self, sim, *, interp="nearest", extrapolation="constant", **kwargs):
+        s2, other, ta = self._unwrap_sim(sim, interp, extrapolation, kwargs)
+        extra = bool(OPTIONS["sdba_extra_output"])
+        nodes = equally_spaced_nodes(self.nquantiles).astype(np.float32)
+        scen, sim_q = device.qdm_adjust(s2, self._af, nodes, _KINDS[self.kind], _INTERP[interp], want_sim_q=extra)
+        out = self._wrap_series(sim, scen, other, ta, "scen", attrs_of(sim))
+        if not extra:
+            return out
+        q = self._wrap_series(sim, sim_q, other, ta, "sim_q",
+                              {"units": "", "long_name": "Percentage rank of sim within its series"})
+        return {"scen": out, "sim_q": q}
