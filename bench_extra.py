@@ -118,6 +118,21 @@ def main():
                                                  _lib.RL_REDUCERS["count"]), a.steps)
         report("spell_runstat window=3 sum<1 count (dry_spell_frequency)", ms, T * C * 4 + P * C * 4,
                cpu=lambda: O.spell_length_statistics(host["pr"], 1.0, 3, "sum", "<", "count", poff))
+    if want("spellmean"):
+        ms = timeit(lambda: device.spell_runstat(pr, poff, 3, _lib.STATS["sum"], _lib.OPS["<"], 1.0,
+                                                 _lib.RL_REDUCERS["mean"]), a.steps)
+        report("spell_runstat window=3 sum<1 mean (any-reducer spell_sumw_kernel)", ms, T * C * 4 + P * C * 4,
+               cpu=lambda: O.spell_length_statistics(host["pr"], 1.0, 3, "sum", "<", "mean", poff))
+    if want("spellmin"):
+        ms = timeit(lambda: device.spell_runstat(tas, poff, 5, _lib.STATS["min"], _lib.OPS[">"], 291.15,
+                                                 _lib.RL_REDUCERS["max"]), a.steps)
+        report("spell_runstat window=5 min>291.15 max (spell_runstat4_kernel)", ms, T * C * 4 + P * C * 4,
+               cpu=lambda: O.spell_length_statistics(host["tas"], 291.15, 5, "min", ">", "max", poff))
+    if want("gap"):
+        ms = timeit(lambda: device.period_runstat_gap(pr, poff, _lib.OPS["<"], 1.0, _lib.RL_REDUCERS["max"], 3),
+                    a.steps)
+        report("period_runstat_gap min_gap=3 <1 max (spell_length_statistics min_gap)", ms, T * C * 4 + P * C * 4,
+               cpu=lambda: O.spell_length_statistics(host["pr"], 1.0, 1, None, "<", "max", poff, min_gap=3))
     if want("first"):
         ms = timeit(lambda: device.period_boundary_run(tas, poff, _lib.OPS[">"], 283.15, 5), a.steps)
         report("period_boundary_run first, window=5", ms, T * C * 4 + P * C * 4,

@@ -5,7 +5,7 @@
 // (`tx_tn_days_above`) and indices/generic.py:1002-1073 (`bivariate_count_occurrences`, var_reducer
 // all / any).  Same lane-owns-4-cells streaming as period_stats.cu with two 128-bit loads per step;
 // operators and the reducer are runtime switches (the kernel moves 8 B per element and is HBM-bound).
-#include "common.cuh"
+#include "runstat.cuh"
 
 namespace xc {
 namespace {
@@ -33,14 +33,8 @@ __device__ __forceinline__ bool cmp_rt(const OpMask& m, float x, float t) {
   return r != m.N;
 }
 
-struct Acc {
-  int cur, mx, mn, sum, cnt;
-  unsigned long long sq;
-  bool skip;
-};
-
-// RED: XC_RL_MAX / SUM / COUNT get branch-free single-accumulator updates (the heat-wave indices);
-// any other value keeps every accumulator and switches on `reducer` at the end.
+// RED: XC_RL_MAX / SUM / COUNT keep a single accumulator (the heat-wave indices); kRunAny keeps every
+// accumulator and picks `reducer` at the end.
 // GTGT: both operators are ">" (the heat-wave indices and tx_tn_days_above): two compares and one
 // predicate op per element pair instead of the six + six of the operator masks.
 template <int VEC, int RED, bool GTGT>
@@ -52,9 +46,11 @@ period_runstat2_kernel(const float* __restrict__ x1, const float* __restrict__ x
   if (c0 >= C) return;
   const int p = blockIdx.y;
   const int t0 = poff[p], tend = poff[p + 1];
-  Acc a[VEC];
+  int cur[VEC];
+  bool skip[VEC];
+  RunAcc<RED> acc[VEC];
 #pragma unroll
-  for (int i = 0; i < VEC; ++i) a[i] = Acc{0, 0, 0x7fffffff, 0, 0, 0ull, false};
+  for (int i = 0; i < VEC; ++i) { cur[i] = 0; skip[i] = false; acc[i].init(); }
   auto cond = [&](float u, float v) -> bool {
     bool c1, c2;
     if constexpr (GTGT) {
@@ -65,26 +61,6 @@ period_runstat2_kernel(const float* __restrict__ x1, const float* __restrict__ x
       c2 = cmp_rt(op2, v, t2);
     }
     return any ? (c1 | c2) : (c1 & c2);
-  };
-  auto close_run = [&](Acc& s) {
-    const int L = s.cur;
-    const bool take = L >= window;
-    if constexpr (RED == XC_RL_MAX) {
-      s.mx = take ? max(s.mx, L) : s.mx;
-    } else if constexpr (RED == XC_RL_SUM) {
-      s.sum += take ? L : 0;
-    } else if constexpr (RED == XC_RL_COUNT) {
-      s.cnt += take ? 1 : 0;
-    } else {
-      if (take) {
-        s.mx = max(s.mx, L);
-        s.mn = min(s.mn, L);
-        s.sum += L;
-        s.cnt += 1;
-        s.sq += (unsigned long long)L * (unsigned long long)L;
-      }
-    }
-    s.cur = 0;
   };
   auto load = [&](const float* base, int t, float (&v)[VEC]) {
     if constexpr (VEC == 4) {
@@ -99,7 +75,7 @@ period_runstat2_kernel(const float* __restrict__ x1, const float* __restrict__ x
     load(x1, t0 - 1, u);
     load(x2, t0 - 1, v);
 #pragma unroll
-    for (int i = 0; i < VEC; ++i) a[i].skip = cond(u[i], v[i]);
+    for (int i = 0; i < VEC; ++i) skip[i] = cond(u[i], v[i]);
   }
   auto step = [&](const float (&u)[VEC], const float (&v)[VEC], bool only_open) {
 #pragma unroll
@@ -107,24 +83,15 @@ period_runstat2_kernel(const float* __restrict__ x1, const float* __restrict__ x
       bool m = cond(u[i], v[i]);
       if (after) {
         if (only_open) {
-          m = m && (a[i].cur > 0);
+          m = m && (cur[i] > 0);
         } else {
-          a[i].skip = a[i].skip && m;
-          m = m && !a[i].skip;
+          skip[i] = skip[i] && m;
+          m = m && !skip[i];
         }
       }
-      if constexpr (RED == XC_RL_MAX || RED == XC_RL_SUM || RED == XC_RL_COUNT) {
-        // branch-free: closing an empty run (cur == 0 < window) is a no-op
-        Acc closing = a[i];
-        close_run(closing);
-        const int next = a[i].cur + 1;
-        a[i].mx = m ? a[i].mx : closing.mx;
-        a[i].sum = m ? a[i].sum : closing.sum;
-        a[i].cnt = m ? a[i].cnt : closing.cnt;
-        a[i].cur = m ? next : 0;
-      } else {
-        if (m) a[i].cur += 1; else close_run(a[i]);
-      }
+      const int L = cur[i];
+      acc[i].add(L, !m && L >= window);
+      cur[i] = m ? L + 1 : 0;
     }
   };
   int t = t0;
@@ -144,7 +111,7 @@ period_runstat2_kernel(const float* __restrict__ x1, const float* __restrict__ x
   if (after) {
     bool open = false;
 #pragma unroll
-    for (int i = 0; i < VEC; ++i) open = open || (a[i].cur > 0);
+    for (int i = 0; i < VEC; ++i) open = open || (cur[i] > 0);
     while (open && t < (int)T) {
       float u[VEC], v[VEC];
       load(x1, t, u);
@@ -152,28 +119,15 @@ period_runstat2_kernel(const float* __restrict__ x1, const float* __restrict__ x
       step(u, v, true);
       open = false;
 #pragma unroll
-      for (int i = 0; i < VEC; ++i) open = open || (a[i].cur > 0);
+      for (int i = 0; i < VEC; ++i) open = open || (cur[i] > 0);
       ++t;
     }
   }
   float res[VEC];
 #pragma unroll
   for (int i = 0; i < VEC; ++i) {
-    close_run(a[i]);
-    const Acc& s = a[i];
-    switch (reducer) {
-      case XC_RL_MAX: res[i] = (float)s.mx; break;
-      case XC_RL_MIN: res[i] = s.cnt ? (float)s.mn : 0.f; break;
-      case XC_RL_SUM: res[i] = (float)s.sum; break;
-      case XC_RL_COUNT: res[i] = (float)s.cnt; break;
-      case XC_RL_MEAN: res[i] = s.cnt ? (float)((double)s.sum / (double)s.cnt) : 0.f; break;
-      default: {
-        if (!s.cnt) { res[i] = 0.f; break; }
-        const double n = (double)s.cnt, mean = (double)s.sum / n;
-        const double var = (double)s.sq / n - mean * mean;
-        res[i] = (float)sqrt(var > 0.0 ? var : 0.0);
-      }
-    }
+    acc[i].add(cur[i], cur[i] >= window);   // the run closed by the period / series end
+    res[i] = acc[i].result(reducer);
   }
   if constexpr (VEC == 4) {
     *reinterpret_cast<float4*>(out + (int64_t)p * C + c0) = make_float4(res[0], res[1], res[2], res[3]);
@@ -218,10 +172,10 @@ extern "C" int32_t xc_period_runstat2_f32(const float* x1, const float* x2, int6
       case XC_RL_MAX: XC_LAUNCH2(4, XC_RL_MAX); break;
       case XC_RL_SUM: XC_LAUNCH2(4, XC_RL_SUM); break;
       case XC_RL_COUNT: XC_LAUNCH2(4, XC_RL_COUNT); break;
-      default: XC_LAUNCH2(4, XC_RL_STD);
+      default: XC_LAUNCH2(4, kRunAny);
     }
   } else {
-    XC_LAUNCH2(1, XC_RL_STD);
+    XC_LAUNCH2(1, kRunAny);
   }
 #undef XC_LAUNCH2
   return launch_status("period_runstat2_kernel");

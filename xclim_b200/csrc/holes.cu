@@ -17,7 +17,7 @@
 // whether a gap open at the period start can still be bridged, walks the period keeping the in-period
 // steps of the unresolved gap pending, and looks ahead at most min_gap-1 steps past the period end
 // to resolve a gap that is still open there.
-#include "common.cuh"
+#include "runstat.cuh"
 
 namespace xc {
 namespace {
@@ -45,18 +45,8 @@ period_runstat_gap_kernel(const float* __restrict__ x, int64_t T, int64_t C, int
     if (t < 0) since = min_gap;  // the series starts inside this gap (or at t0): never bridged
   }
   int cur = 0, pend = 0;
-  int mx = 0, mn = 0x7fffffff, sum = 0, cnt = 0;
-  unsigned long long sq = 0ull;
-  auto close_run = [&]() {
-    if (cur >= window) {
-      mx = max(mx, cur);
-      mn = min(mn, cur);
-      sum += cur;
-      cnt += 1;
-      sq += (unsigned long long)cur * (unsigned long long)cur;
-    }
-    cur = 0;
-  };
+  RunAcc<kRunAny> acc;
+  acc.init();
   for (int t = t0; t < t1; ++t) {
     if (m_at(t)) {
       if (since < min_gap) cur += pend;  // the gap just closed was short: its steps count as spell steps
@@ -69,7 +59,8 @@ period_runstat_gap_kernel(const float* __restrict__ x, int64_t T, int64_t C, int
         if (since < min_gap) {
           ++pend;                         // still bridgeable
         } else {                          // the gap reached min_gap: the run ended before it
-          close_run();
+          acc.add(cur, cur >= window);
+          cur = 0;
           pend = 0;
         }
       }
@@ -86,22 +77,8 @@ period_runstat_gap_kernel(const float* __restrict__ x, int64_t T, int64_t C, int
     }
     if (bridged) cur += pend;
   }
-  close_run();
-  float res;
-  switch (reducer) {
-    case XC_RL_MAX: res = (float)mx; break;
-    case XC_RL_MIN: res = cnt ? (float)mn : 0.f; break;
-    case XC_RL_SUM: res = (float)sum; break;
-    case XC_RL_COUNT: res = (float)cnt; break;
-    case XC_RL_MEAN: res = cnt ? (float)((double)sum / (double)cnt) : 0.f; break;
-    default: {
-      if (!cnt) { res = 0.f; break; }
-      const double n = (double)cnt, mean = (double)sum / n;
-      const double var = (double)sq / n - mean * mean;
-      res = (float)sqrt(var > 0.0 ? var : 0.0);
-    }
-  }
-  out[(int64_t)p * C + c] = res;
+  acc.add(cur, cur >= window);
+  out[(int64_t)p * C + c] = acc.result(reducer);
 }
 
 }  // namespace

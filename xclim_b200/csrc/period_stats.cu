@@ -20,7 +20,7 @@
 // flight; data is read exactly once (ld.global.nc.L1::no_allocate).
 #include <type_traits>
 
-#include "common.cuh"
+#include "runstat.cuh"
 
 namespace xc {
 namespace {
@@ -110,42 +110,6 @@ period_count_kernel(const float* __restrict__ x, int64_t C, int64_t ldx,
 // ------------------------------------------------------------------------------------------------
 // run-length statistics
 // ------------------------------------------------------------------------------------------------
-// Per-cell accumulator over the run lengths L >= window attributed to the period.
-template <int RED>
-struct RunAcc {
-  int32_t a;        // MAX: max L ; MIN: min L ; SUM: sum L ; COUNT/MEAN/STD: n runs
-  int32_t s;        // MEAN/STD: sum L
-  unsigned long long q;  // STD: sum L^2
-  __device__ __forceinline__ void init() {
-    a = (RED == XC_RL_MIN) ? 0x7fffffff : 0;
-    s = 0;
-    q = 0ull;
-  }
-  __device__ __forceinline__ void add(int32_t L, bool take) {
-    if constexpr (RED == XC_RL_MAX) a = take ? max(a, L) : a;
-    if constexpr (RED == XC_RL_MIN) a = take ? min(a, L) : a;
-    if constexpr (RED == XC_RL_SUM) a += take ? L : 0;
-    if constexpr (RED == XC_RL_COUNT) a += take ? 1 : 0;
-    if constexpr (RED == XC_RL_MEAN || RED == XC_RL_STD) {
-      a += take ? 1 : 0;
-      s += take ? L : 0;
-    }
-    if constexpr (RED == XC_RL_STD) q += take ? (unsigned long long)L * (unsigned long long)L : 0ull;
-  }
-  __device__ __forceinline__ float result() const {
-    if constexpr (RED == XC_RL_MAX || RED == XC_RL_SUM || RED == XC_RL_COUNT) return (float)a;
-    if constexpr (RED == XC_RL_MIN) return a == 0x7fffffff ? 0.f : (float)a;
-    if constexpr (RED == XC_RL_MEAN) return a == 0 ? 0.f : (float)((double)s / (double)a);
-    if constexpr (RED == XC_RL_STD) {
-      if (a == 0) return 0.f;
-      double n = (double)a, m = (double)s / n;
-      double var = (double)q / n - m * m;
-      return (float)sqrt(var > 0.0 ? var : 0.0);
-    }
-    return 0.f;
-  }
-};
-
 // FASTMAX: reducer == max and window == 1 needs no run-end detection: max over t of the running
 // length (this is the maximum_consecutive_dry_days configuration).
 template <int OP, int RED, int VEC, bool VALID, bool AFTER, bool FASTMAX>
@@ -367,6 +331,7 @@ period_reduce_kernel(const float* __restrict__ x, int64_t C, int64_t ldx,
     if constexpr (STAT == XC_STAT_MEAN) res[i] = n[i] ? (float)(s[i] / nn) : NAN;
     if constexpr (STAT == XC_STAT_MIN || STAT == XC_STAT_MAX) res[i] = n[i] ? m[i] : NAN;
     if constexpr (STAT == XC_STAT_STD || STAT == XC_STAT_VAR) {
+      // stat_result()'s formula, kept as a copy: calling it reorders the register allocation of this kernel
       if (n[i] == 0) {
         res[i] = NAN;
       } else {

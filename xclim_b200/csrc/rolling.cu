@@ -11,7 +11,7 @@
 // window are re-read from L1/L2 (the rows were just fetched by the same warp), so DRAM traffic stays
 // one read of the input.  These are the low-volume members of the family (the window == 1 fast
 // kernels in period_stats.cu carry the headline configurations); operators are runtime switches.
-#include "common.cuh"
+#include "runstat.cuh"
 #include <limits>
 #include <type_traits>
 #include <string.h>
@@ -21,6 +21,8 @@ namespace {
 
 constexpr int kThreads = 128;
 
+// A switch on the uniform operator, not bivariate.cu's branch-free OpMask: with the mask form the
+// compute-bound spell_runstat4_kernel runs about 14% slower.
 __device__ __forceinline__ bool cmp_rt(int op, float x, float t) {
   switch (op) {
     case XC_OP_GT: return x > t;
@@ -82,17 +84,8 @@ rolling_period_reduce_kernel(const float* __restrict__ x, int64_t T, int64_t C, 
   const int p = blockIdx.y;
   const int t0 = poff[p], t1 = poff[p + 1];
   const float* col = x + c;
-  double s = 0.0, q = 0.0;
-  float m = (stat == XC_STAT_MIN) ? INFINITY : -INFINITY;
-  int n = 0;
-  auto take = [&](float r) {
-    if (r == r) {
-      ++n;
-      s += (double)r;
-      q += (double)r * (double)r;
-      m = (stat == XC_STAT_MIN) ? fminf(m, r) : fmaxf(m, r);
-    }
-  };
+  StatAcc acc;
+  acc.init(stat);
   // the value labelled t covers x[i .. i+w-1], i = t + shift - w + 1 (shift 0: right-aligned, w/2: centred)
   if (wstat == XC_STAT_SUM || wstat == XC_STAT_MEAN) {
     const double inv = (wstat == XC_STAT_MEAN) ? 1.0 / (double)w : 1.0;
@@ -104,7 +97,7 @@ rolling_period_reduce_kernel(const float* __restrict__ x, int64_t T, int64_t C, 
     if (t < t1 && i + w <= (int)T)
       for (int k = 0; k < w; ++k) win.add(__ldg(col + (int64_t)(i + k) * ldx));
     while (t < t1 && i + w <= (int)T) {
-      take(win.nan ? NAN : (float)(wstat == XC_STAT_MEAN ? win.s / (double)w : win.s));
+      acc.take(win.nan ? NAN : (float)(wstat == XC_STAT_MEAN ? win.s / (double)w : win.s));
       // slide by up to kChunk steps with all loads issued first
       const int steps = min(kChunk, min(t1 - 1 - t, (int)T - (i + w)));
       if (steps <= 0) break;
@@ -121,7 +114,7 @@ rolling_period_reduce_kernel(const float* __restrict__ x, int64_t T, int64_t C, 
         if (k < steps) {
           win.add(vin[k]);
           win.drop(vout[k]);
-          if (k + 1 < steps) take(win.nan ? NAN : (float)(wstat == XC_STAT_MEAN ? win.s / (double)w : win.s));
+          if (k + 1 < steps) acc.take(win.nan ? NAN : (float)(wstat == XC_STAT_MEAN ? win.s / (double)w : win.s));
         }
       }
       t += steps;
@@ -133,26 +126,10 @@ rolling_period_reduce_kernel(const float* __restrict__ x, int64_t T, int64_t C, 
       const int i = t + shift - w + 1;
       float r = NAN;
       if (i >= 0 && i + w <= (int)T) r = window_stat(col, ldx, i, w, wstat);
-      take(r);
+      acc.take(r);
     }
   }
-  float res;
-  const double nn = (double)n;
-  switch (stat) {
-    case XC_STAT_SUM: res = (float)s; break;
-    case XC_STAT_COUNT: res = (float)n; break;
-    case XC_STAT_MEAN: res = n ? (float)(s / nn) : NAN; break;
-    case XC_STAT_MIN:
-    case XC_STAT_MAX: res = n ? m : NAN; break;
-    default: {
-      if (!n) { res = NAN; break; }
-      const double mean = s / nn;
-      double var = q / nn - mean * mean;
-      var = var > 0.0 ? var : 0.0;
-      res = (stat == XC_STAT_STD) ? (float)sqrt(var) : (float)var;
-    }
-  }
-  out[(int64_t)p * C + c] = res;
+  out[(int64_t)p * C + c] = acc.result(stat);
 }
 
 // mask[t] = any length-w block [i, i+w-1] containing t, fully inside the series, whose window
@@ -224,15 +201,15 @@ spell_runstat_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t 
   };
   bool skip = false;
   if (after && t0 > 0) skip = mask_at(t0 - 1);  // a run already open belongs to an earlier period
-  int cur = 0, mx = 0, mn = 0x7fffffff, sum = 0, cnt = 0;
-  unsigned long long sq = 0ull;
-  auto close_run = [&](int L) {
-    if (L >= 1) {
-      mx = max(mx, L);
-      mn = min(mn, L);
-      sum += L;
-      cnt += 1;
-      sq += (unsigned long long)L * (unsigned long long)L;
+  int cur = 0;
+  RunAcc<kRunAny> acc;
+  acc.init();
+  auto step = [&](bool m) {
+    if (m) {
+      ++cur;
+    } else {
+      acc.add(cur, cur >= 1);
+      cur = 0;
     }
   };
   for (int t = t0; t < t1; ++t) {
@@ -241,41 +218,13 @@ spell_runstat_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t 
       skip = skip && m;
       m = m && !skip;
     }
-    if (m) {
-      ++cur;
-    } else {
-      close_run(cur);
-      cur = 0;
-    }
+    step(m);
   }
   if (after) {
-    int t = t1;
-    while (cur > 0 && t < (int)T) {
-      if (mask_at(t)) {
-        ++cur;
-      } else {
-        close_run(cur);
-        cur = 0;
-      }
-      ++t;
-    }
+    for (int t = t1; cur > 0 && t < (int)T; ++t) step(mask_at(t));
   }
-  close_run(cur);
-  float res;
-  switch (reducer) {
-    case XC_RL_MAX: res = (float)mx; break;
-    case XC_RL_MIN: res = cnt ? (float)mn : 0.f; break;
-    case XC_RL_SUM: res = (float)sum; break;
-    case XC_RL_COUNT: res = (float)cnt; break;
-    case XC_RL_MEAN: res = cnt ? (float)((double)sum / (double)cnt) : 0.f; break;
-    default: {
-      if (!cnt) { res = 0.f; break; }
-      const double n = (double)cnt, mean = (double)sum / n;
-      double var = (double)sq / n - mean * mean;
-      res = (float)sqrt(var > 0.0 ? var : 0.0);
-    }
-  }
-  out[(int64_t)p * C + c] = res;
+  acc.add(cur, cur >= 1);
+  out[(int64_t)p * C + c] = acc.result(reducer);
 }
 
 
@@ -367,11 +316,9 @@ rolling_period_reduce4_kernel(const float* __restrict__ x, int64_t T, int64_t C,
   const int p = blockIdx.y;
   const int t0 = poff[p], t1 = poff[p + 1];
   const float* col = x + c;
-  double s[4] = {0, 0, 0, 0}, q[4] = {0, 0, 0, 0};
-  float m[4];
-  int n[4] = {0, 0, 0, 0};
+  StatAcc acc[4];
 #pragma unroll
-  for (int j = 0; j < 4; ++j) m[j] = (stat == XC_STAT_MIN) ? INFINITY : -INFINITY;
+  for (int j = 0; j < 4; ++j) acc[j].init(stat);
   // the value labelled t covers the w rows ending at e = t + shift; incomplete windows give NaN (ignored)
   const int eb = max(t0 + shift, w - 1);
   const int ee = min((int)T - 1, t1 - 1 + shift);
@@ -394,37 +341,12 @@ rolling_period_reduce4_kernel(const float* __restrict__ x, int64_t T, int64_t C,
         float r[4];
         window_stat4(win, ring4, lane, w, wstat, r);
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          if (r[j] == r[j]) {
-            ++n[j];
-            s[j] += (double)r[j];
-            q[j] += (double)r[j] * (double)r[j];
-            m[j] = (stat == XC_STAT_MIN) ? fminf(m[j], r[j]) : fmaxf(m[j], r[j]);
-          }
-        }
+        for (int j = 0; j < 4; ++j) acc[j].take(r[j]);
       }
     }
   }
-  float res[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const double nn = (double)n[j];
-    switch (stat) {
-      case XC_STAT_SUM: res[j] = (float)s[j]; break;
-      case XC_STAT_COUNT: res[j] = (float)n[j]; break;
-      case XC_STAT_MEAN: res[j] = n[j] ? (float)(s[j] / nn) : NAN; break;
-      case XC_STAT_MIN:
-      case XC_STAT_MAX: res[j] = n[j] ? m[j] : NAN; break;
-      default: {
-        if (!n[j]) { res[j] = NAN; break; }
-        const double mean = s[j] / nn;
-        double var = q[j] / nn - mean * mean;
-        var = var > 0.0 ? var : 0.0;
-        res[j] = (stat == XC_STAT_STD) ? (float)sqrt(var) : (float)var;
-      }
-    }
-  }
-  *reinterpret_cast<float4*>(out + (int64_t)p * C + c) = make_float4(res[0], res[1], res[2], res[3]);
+  *reinterpret_cast<float4*>(out + (int64_t)p * C + c) =
+      make_float4(acc[0].result(stat), acc[1].result(stat), acc[2].result(stat), acc[3].result(stat));
 }
 
 // Spell statistics, streaming form.  cond(e) = (statistic of the w rows ending at e) op thr;
@@ -446,20 +368,10 @@ spell_runstat4_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t
   const int first_t = (AFTER && t0 > 0) ? t0 - 1 : t0;
   int last[4] = {-1, -1, -1, -1};
   bool skip[4] = {false, false, false, false};
-  int cur[4] = {0, 0, 0, 0}, mx[4] = {0, 0, 0, 0}, sum[4] = {0, 0, 0, 0}, cnt[4] = {0, 0, 0, 0};
-  int mn[4] = {0x7fffffff, 0x7fffffff, 0x7fffffff, 0x7fffffff};
-  unsigned long long sq[4] = {0ull, 0ull, 0ull, 0ull};
-  auto close_run = [&](int j) {
-    const int L = cur[j];
-    if (L >= 1) {
-      mx[j] = max(mx[j], L);
-      mn[j] = min(mn[j], L);
-      sum[j] += L;
-      cnt[j] += 1;
-      sq[j] += (unsigned long long)L * (unsigned long long)L;
-    }
-    cur[j] = 0;
-  };
+  int cur[4] = {0, 0, 0, 0};
+  RunAcc<kRunAny> acc[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) acc[j].init();
   // mask value of step t for cell j (t >= first_t, in time order)
   auto feed = [&](int j, int t, bool mk) {
     if (AFTER) {
@@ -471,8 +383,12 @@ spell_runstat4_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t
         return;                              // past the period end only an open run is followed
       }
     }
-    if (mk) ++cur[j];
-    else close_run(j);
+    if (mk) {
+      ++cur[j];
+    } else {
+      acc[j].add(cur[j], cur[j] >= 1);
+      cur[j] = 0;
+    }
   };
   auto open_any = [&]() { return (cur[0] | cur[1] | cur[2] | cur[3]) != 0; };
 
@@ -518,20 +434,8 @@ spell_runstat4_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t
   float res[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    close_run(j);
-    switch (reducer) {
-      case XC_RL_MAX: res[j] = (float)mx[j]; break;
-      case XC_RL_MIN: res[j] = cnt[j] ? (float)mn[j] : 0.f; break;
-      case XC_RL_SUM: res[j] = (float)sum[j]; break;
-      case XC_RL_COUNT: res[j] = (float)cnt[j]; break;
-      case XC_RL_MEAN: res[j] = cnt[j] ? (float)((double)sum[j] / (double)cnt[j]) : 0.f; break;
-      default: {
-        if (!cnt[j]) { res[j] = 0.f; break; }
-        const double nn = (double)cnt[j], mean = (double)sum[j] / nn;
-        double var = (double)sq[j] / nn - mean * mean;
-        res[j] = (float)sqrt(var > 0.0 ? var : 0.0);
-      }
-    }
+    acc[j].add(cur[j], cur[j] >= 1);
+    res[j] = acc[j].result(reducer);
   }
   *reinterpret_cast<float4*>(out + (int64_t)p * C + c) = make_float4(res[0], res[1], res[2], res[3]);
 }
@@ -586,33 +490,29 @@ spell_sumw_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t ldx
     for (int j = 0; j < 4; ++j) ring[k][j] = 0.0;
   int last[4] = {-1, -1, -1, -1};
   bool skip[4] = {false, false, false, false};
-  int cur[4] = {0, 0, 0, 0}, mx[4] = {0, 0, 0, 0}, sum[4] = {0, 0, 0, 0}, cnt[4] = {0, 0, 0, 0};
-  int mn[4] = {0x7fffffff, 0x7fffffff, 0x7fffffff, 0x7fffffff};
-  unsigned long long sq[4] = {0ull, 0ull, 0ull, 0ull};
+  // MAX / SUM / COUNT keep a running form in acc.a; any other reducer closes runs into RunAcc<kRunAny>
+  constexpr bool kRunning = RED == XC_RL_MAX || RED == XC_RL_SUM || RED == XC_RL_COUNT;
+  int cur[4] = {0, 0, 0, 0};
+  RunAcc<kRunning ? RED : kRunAny> acc[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) acc[j].init();
   // run-length update with the mask value of the next step (cur > 0 <=> a run is open)
   auto update = [&](int j, bool mk) {
     if constexpr (RED == XC_RL_MAX) {
       cur[j] = mk ? cur[j] + 1 : 0;
-      mx[j] = max(mx[j], cur[j]);
+      acc[j].a = max(acc[j].a, cur[j]);
     } else if constexpr (RED == XC_RL_SUM) {
       cur[j] = mk ? 1 : 0;
-      sum[j] += cur[j];
+      acc[j].a += cur[j];
     } else if constexpr (RED == XC_RL_COUNT) {
       const int now = mk ? 1 : 0;
-      cnt[j] += now & (cur[j] ^ 1);
+      acc[j].a += now & (cur[j] ^ 1);
       cur[j] = now;
+    } else if (mk) {
+      ++cur[j];
     } else {
-      if (mk) {
-        ++cur[j];
-      } else if (cur[j] > 0) {
-        const int L = cur[j];
-        mn[j] = min(mn[j], L);
-        mx[j] = max(mx[j], L);
-        sum[j] += L;
-        cnt[j] += 1;
-        sq[j] += (unsigned long long)L * (unsigned long long)L;
-        cur[j] = 0;
-      }
+      acc[j].add(cur[j], cur[j] > 0);
+      cur[j] = 0;
     }
   };
   // inside the period: with resample_before_rl=False a run that was already open at t0 is skipped
@@ -689,35 +589,8 @@ spell_sumw_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t ldx
   float res[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    if constexpr (RED == XC_RL_MAX) {
-      res[j] = (float)mx[j];
-    } else if constexpr (RED == XC_RL_SUM) {
-      res[j] = (float)sum[j];
-    } else if constexpr (RED == XC_RL_COUNT) {
-      res[j] = (float)cnt[j];
-    } else {
-      if (cur[j] > 0) {
-        const int L = cur[j];
-        mn[j] = min(mn[j], L);
-        mx[j] = max(mx[j], L);
-        sum[j] += L;
-        cnt[j] += 1;
-        sq[j] += (unsigned long long)L * (unsigned long long)L;
-      }
-      switch (reducer) {
-        case XC_RL_MIN: res[j] = cnt[j] ? (float)mn[j] : 0.f; break;
-        case XC_RL_MEAN: res[j] = cnt[j] ? (float)((double)sum[j] / (double)cnt[j]) : 0.f; break;
-        case XC_RL_MAX: res[j] = (float)mx[j]; break;
-        case XC_RL_SUM: res[j] = (float)sum[j]; break;
-        case XC_RL_COUNT: res[j] = (float)cnt[j]; break;
-        default: {
-          if (!cnt[j]) { res[j] = 0.f; break; }
-          const double nn = (double)cnt[j], mean = (double)sum[j] / nn;
-          double var = (double)sq[j] / nn - mean * mean;
-          res[j] = (float)sqrt(var > 0.0 ? var : 0.0);
-        }
-      }
-    }
+    if constexpr (!kRunning) acc[j].add(cur[j], cur[j] > 0);   // the run closed by the period / series end
+    res[j] = acc[j].result(reducer);
   }
   *reinterpret_cast<float4*>(out + (int64_t)p * C + c) = make_float4(res[0], res[1], res[2], res[3]);
 }
@@ -792,6 +665,7 @@ rolling_sumw_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t l
   float res[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
+    // stat_result()'s formula, kept as a copy: calling it changes this kernel's code
     const double nn = (double)n[j];
     switch (stat) {
       case XC_STAT_SUM: res[j] = (float)s[j]; break;
@@ -873,7 +747,7 @@ int32_t launch_spell_sumw_red(const float* x, int64_t T, int64_t C, int64_t ldx,
     case XC_RL_MAX: spell_sumw_kernel<W, XC_RL_MAX, AFTER><<<grid, kThreads, 0, st>>>(x, T, C, ldx, poff, g, reducer, out); break;
     case XC_RL_SUM: spell_sumw_kernel<W, XC_RL_SUM, AFTER><<<grid, kThreads, 0, st>>>(x, T, C, ldx, poff, g, reducer, out); break;
     case XC_RL_COUNT: spell_sumw_kernel<W, XC_RL_COUNT, AFTER><<<grid, kThreads, 0, st>>>(x, T, C, ldx, poff, g, reducer, out); break;
-    default: spell_sumw_kernel<W, XC_RL_STD, AFTER><<<grid, kThreads, 0, st>>>(x, T, C, ldx, poff, g, reducer, out);
+    default: spell_sumw_kernel<W, kRunAny, AFTER><<<grid, kThreads, 0, st>>>(x, T, C, ldx, poff, g, reducer, out);
   }
   return launch_status("spell_sumw_kernel");
 }
@@ -977,38 +851,15 @@ rolling_period_reduce_sel_kernel(const float* __restrict__ x, int64_t T, int64_t
   const int p = blockIdx.y;
   const int t0 = poff[p], t1 = poff[p + 1];
   const float* col = x + c;
-  double s = 0.0, q = 0.0;
-  float m = (stat == XC_STAT_MIN) ? INFINITY : -INFINITY;
-  int n = 0;
+  StatAcc acc;
+  acc.init(stat);
   for (int t = t0; t < t1; ++t) {
     if (!keep[t]) continue;
     const int i = t + shift - w + 1;
     if (i < 0 || i + w > (int)T) continue;            // incomplete window: NaN, skipped by the reduction
-    const float r = window_stat(col, ldx, i, w, wstat);
-    if (r == r) {
-      ++n;
-      s += (double)r;
-      q += (double)r * (double)r;
-      m = (stat == XC_STAT_MIN) ? fminf(m, r) : fmaxf(m, r);
-    }
+    acc.take(window_stat(col, ldx, i, w, wstat));
   }
-  float res;
-  const double nn = (double)n;
-  switch (stat) {
-    case XC_STAT_SUM: res = (float)s; break;
-    case XC_STAT_COUNT: res = (float)n; break;
-    case XC_STAT_MEAN: res = n ? (float)(s / nn) : NAN; break;
-    case XC_STAT_MIN:
-    case XC_STAT_MAX: res = n ? m : NAN; break;
-    default: {
-      if (!n) { res = NAN; break; }
-      const double mean = s / nn;
-      double var = q / nn - mean * mean;
-      var = var > 0.0 ? var : 0.0;
-      res = (stat == XC_STAT_STD) ? (float)sqrt(var) : (float)var;
-    }
-  }
-  out[(int64_t)p * C + c] = res;
+  out[(int64_t)p * C + c] = acc.result(stat);
 }
 
 }  // namespace
