@@ -232,6 +232,25 @@ def main():
                    2 * T * C * 4 + 20 * C * 4 + (T * C * 8 if with_q else 0),
                    {"scratch_bytes_per_cell": 6 * T + 16},
                    cpu=lambda: QO.qdm_adjust(host["hist"], qaf, "+", "linear"))
+    if want("dqm"):
+        hist = af = hq = None
+        hist = device.synth(T, C, kind=1, seed=5, cells_per_lat=X, n_lat_global=a.lat)
+        if a.cpu:
+            from oracle import dqm_oracle as DO
+            host["hist"] = hist[:, :S].cpu().numpy()
+        ms_mean = timeit(lambda: device.period_reduce(tas, [0, T], _lib.STATS["mean"]), a.steps)
+        ms = timeit(lambda: device.dqm_train(tas, hist, 20, 0), a.steps)
+        report("dqm_train nq=20 (means pass + selection on the normalised series)", ms, 2 * T * C * 4,
+               {"means_pass_ms_each": ms_mean, "means_pass_algorithmic_bytes": 2 * T * C * 4},
+               cpu=lambda: DO.dqm_train(host["tas"], host["hist"], 20, "+"))
+        af, hq, sc = device.dqm_train(tas, hist, 20, 0)
+        if a.cpu:
+            daf, dhq, dsc = (v[..., :S].cpu().numpy() for v in (af, hq, sc))
+        ms_fit = timeit(lambda: device.poly_fit(hist, 1, 0, sc), a.steps)
+        ms = timeit(lambda: device.dqm_adjust(hist, af, hq, sc, 0, 1, 1), a.steps)
+        report("dqm_adjust linear nq=20 detrend=1 (trend fit + apply, sim -> scen)", ms, 3 * T * C * 4,
+               {"fit_ms": ms_fit},
+               cpu=lambda: DO.dqm_adjust(host["hist"], daf, dhq, dsc, "+", "linear", detrend=1))
     if want("fwi") and a.only:      # the fire-weather kernel: opt-in (--only fwi), never part of a default run
         import time
 

@@ -371,6 +371,43 @@ int32_t xc_qdm_adjust_f32(const float* sim, int64_t T, int64_t C, int64_t ldx,
                           void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * a20 (cont.)  detrended quantile mapping -- xsdba.DetrendedQuantileMapping (third-party,
+ *   re-exported by sdba.py:11; xsdba's dqm_train / dqm_adjust with PolyDetrend), group="time",
+ *   extrapolation="constant"; and the polynomial trend of xclim.indices.generic.detrend
+ *   (indices/generic.py:1711-1736: polyfit, then polyval).  kind 0 = "+", 1 = "*"; (+) is + or *,
+ *   inv(m) is -m or float32(1 / m).
+ *   train, per cell of ref, hist (T, C):
+ *     m_ref, m_hist = NaN-skipping means (float64 sums over n, rounded once: xc_period_reduce_f32,
+ *       one period, XC_STAT_MEAN); scaling[c] = m_ref - m_hist or m_ref / m_hist (float32);
+ *     af, hist_q (nq, C) = xc_eqm_train_f32 of refn = float32(ref (+) inv(m_ref)) and histn (likewise),
+ *       computed without a normalised copy of ref / hist.
+ *     workspace: device scratch of at least xc_dqm_train_workspace_bytes(T, C, nq).  T <= 32768.
+ *   trend of a series y with degree D in {0, 1, 2}: the least-squares polynomial over the valid steps
+ *     in the basis u_t = (2t - (T - 1)) / max(T - 1, 1), float64; the degree is lowered to n - 1 for
+ *     n <= D valid steps; all NaN for n = 0 or any infinite valid value.  coef (D + 1, C) float64,
+ *     row k = the coefficient of u^k; tau_t = ((c2 u + c1) u + c0) without fused multiply-adds.
+ *     xc_poly_fit_f32 fits y = x, or y = float32(x (+) scaling[c]) when scaling is not NULL.
+ *   adjust, per cell of sim (T, C), coef = xc_poly_fit_f32(sim, kind, scaling):
+ *     y = float32(sim (+) scaling); d = y - tau or y * (1 / tau) (float64);
+ *     f = interp(d; hist_q -> af) over the entries where neither is NaN (interp 0 = nearest, ties to
+ *       the lower node; 1 = linear, scipy interp1d's two-weight form), constant end factors, float32;
+ *     scen = float32((d (+) f) (+) tau) with the inner operations in float64.
+ *     nq in [2, 200]; no limit on T.
+ *   detrend: out (T, C) float64 = x - tau, with coef = xc_poly_fit_f32(x, scaling = NULL); no limit on T.
+ * ------------------------------------------------------------------------------------------- */
+int64_t xc_dqm_train_workspace_bytes(int64_t T, int64_t C, int32_t nq);
+int32_t xc_dqm_train_f32(const float* ref, const float* hist, int64_t T, int64_t C, int64_t ldx,
+                         int32_t nq, int32_t kind, float* af, float* hist_q, float* scaling,
+                         void* workspace, int64_t workspace_bytes, void* stream);
+int32_t xc_poly_fit_f32(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t degree, int32_t kind,
+                        const float* scaling, double* coef, void* stream);
+int32_t xc_dqm_adjust_f32(const float* sim, int64_t T, int64_t C, int64_t ldx, const float* af,
+                          const float* hist_q, const float* scaling, const double* coef, int32_t nq,
+                          int32_t kind, int32_t interp, int32_t degree, float* scen, void* stream);
+int32_t xc_detrend_apply_f32(const float* x, int64_t T, int64_t C, int64_t ldx, const double* coef,
+                             int32_t degree, double* out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Synthetic inputs (BASELINE.json configs; SURVEY.md section 8d).  Stateless counter-based
  * generators: value(t, global_cell) depends only on (seed, t, global_cell), so a lat tile
  * generated on any rank equals the same slab of the global grid.

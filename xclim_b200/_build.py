@@ -29,8 +29,9 @@ NVCC_FLAGS = [
 ]
 
 
-#: per-file flags.  fwi.cu mirrors numba / numpy arithmetic, which never fuses a multiply with an add.
-EXTRA_FLAGS = {"fwi.cu": ["-fmad=false"]}
+#: per-file flags.  fwi.cu mirrors numba / numpy arithmetic, which never fuses a multiply with an add; so does
+#: dqm.cu (the trend, detrend and retrend of the oracle, operation by operation).
+EXTRA_FLAGS = {"fwi.cu": ["-fmad=false"], "dqm.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:

@@ -60,6 +60,11 @@ SIGNATURES = {
     "xc_eqm_adjust_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "xc_qdm_adjust_workspace_bytes": (_i64, [_i64, _i64]),
     "xc_qdm_adjust_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _i64, _vp]),
+    "xc_dqm_train_workspace_bytes": (_i64, [_i64, _i64, _i32]),
+    "xc_dqm_train_f32": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "xc_poly_fit_f32": (_i32, [_vp, _i64, _i64, _i64, _i32, _i32, _vp, _vp, _vp]),
+    "xc_dqm_adjust_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "xc_detrend_apply_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp]),
     "xc_synth_f32": (_i32, [_vp, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _i32, _u64, _vp]),
     "xc_mask_steps_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _vp]),
     "xc_host_stream_workspace_bytes": (_i64, [_i64, _i64, _vp, _i32]),

@@ -15,12 +15,25 @@
 // gather are shared through L2.  adjust is a streaming pass: a lane owns one cell, keeps the 2*nq
 // table entries of its cell in a conflict-free shared-memory column and does a binary search per
 // element.
+#include <float.h>
 #include <stdlib.h>
 
 #include "common.cuh"
 
 namespace xc {
 namespace {
+
+// DQM trains EQM on mean-normalised series, refn = float32(ref (+|*) c) with c = inv(mean) of the cell (-m for
+// "+", float32(1 / m) for "*"; dqm.cu).  The train kernels take c from `norm` [2][C] (ref, then hist) under the
+// template flag NORM instead of reading a second, normalised copy of ref and hist.
+__device__ __forceinline__ float norm_apply(float x, int32_t kind, float c) {
+  return kind == 0 ? __fadd_rn(x, c) : __fmul_rn(x, c);
+}
+// x -> norm_apply(x, kind, c) is non-decreasing and never makes a NaN: then the order statistics of the normalised
+// series are the normalised order statistics of the raw one ("+" with a finite c, "*" with a normal positive c)
+__device__ __forceinline__ bool norm_monotone(int32_t kind, float c) {
+  return kind == 0 ? fabsf(c) < INFINITY : (c >= FLT_MIN && c < INFINITY);
+}
 
 constexpr int kSortThreads = 256;
 constexpr int kBins = 1024;      // histogram bins over [min, max] of the series
@@ -33,11 +46,12 @@ constexpr int kMaxTargets = 128; // order statistics per series (2 per quantile)
 // wanted order statistic from the prefix sums, (3) gathers only the elements of those bins and (4)
 // ranks them by counting.  Degenerate distributions (a wanted bin with more than kCap elements that
 // are not all equal, e.g. heavy ties next to other values) fall back to the full bitonic sort.
-template <int NPAD>
+// NORM (DQM): every element is normalised on load, before anything else sees it.
+template <int NPAD, bool NORM>
 __global__ void __launch_bounds__(kSortThreads)
 eqm_train_kernel(const float* __restrict__ ref, const float* __restrict__ hist, int32_t T, int64_t C, int64_t ldx,
                  int32_t nq, int32_t kind, float* __restrict__ af, float* __restrict__ hist_q,
-                 const int32_t* __restrict__ redo = nullptr) {
+                 const int32_t* __restrict__ redo, const float* __restrict__ norm) {
   extern __shared__ float keys[];             // NPAD keys | nq ref quantiles | candidate lists
   float* refq = keys + NPAD;
   float* cand = refq + ((nq + 3) & ~3);       // [2 * nq][kCap]
@@ -61,8 +75,11 @@ eqm_train_kernel(const float* __restrict__ ref, const float* __restrict__ hist, 
     // ---- load, count valid, min / max
     float mn = INFINITY, mx = -INFINITY;
     int nvalid = 0;
+    float nc = 0.f;
+    if constexpr (NORM) nc = norm[(int64_t)pass * C + c];
     for (int t = tid; t < T; t += kSortThreads) {
-      const float v = ld_stream(src + (int64_t)t * ldx);
+      float v = ld_stream(src + (int64_t)t * ldx);
+      if constexpr (NORM) v = norm_apply(v, kind, nc);
       keys[t] = v;
       if (v == v) { mn = fminf(mn, v); mx = fmaxf(mx, v); ++nvalid; }
     }
@@ -258,6 +275,11 @@ eqm_train_kernel(const float* __restrict__ ref, const float* __restrict__ hist, 
 // those of eqm_train_kernel bit for bit.
 // Instantiations: <32, 1024> default; <32, 512>; <16, 512> when C is a multiple of 16 only or the targets of
 // 32 cells do not fit (nq > 40).
+// NORM (DQM): the ranks are selected on the raw series and the two order statistics of a quantile (or the
+// constant of a degenerate cell) are normalised before the lerp, which equals selecting them on the normalised
+// series when the transform is monotone (norm_monotone).  Cells where it is not, and cells where the raw or the
+// normalised range is infinite (the one-cell kernel's degenerate test could differ), go to the redo list, whose
+// kernel normalises on load.
 // ------------------------------------------------------------------------------------------------
 constexpr int kPool = 1024;                 // candidate floats per cell (the same words hold the histogram first)
 constexpr int kHeavy = 192;                 // bins above this must be constant
@@ -287,11 +309,12 @@ __host__ __device__ inline size_t train_group_smem_bytes(int kG, int ntg) {
          + (size_t)kG * ntg * (4 * 8);     // tgt_rank, tgt_bin, tgt_val, slot_bin, slot_off, slot_n, slot_min / max (2)
 }
 
-template <int kG, int kGT>
+template <int kG, int kGT, bool NORM>
 __global__ void __launch_bounds__(kGT, 1)
 eqm_train_group_kernel(const float* __restrict__ ref, const float* __restrict__ hist, int32_t T, int64_t C,
                        int64_t ldx, int32_t nq, int32_t kind, float* __restrict__ af, float* __restrict__ hist_q,
-                       int32_t* __restrict__ redo /* [0] = count, then cell indexes */) {
+                       int32_t* __restrict__ redo /* [0] = count, then cell indexes */,
+                       const float* __restrict__ norm) {
   extern __shared__ __align__(16) unsigned char smg[];
   const int ntg = 2 * nq;
   constexpr int kSub = kG / 4;       // threads (128-bit loads) per time row
@@ -372,6 +395,14 @@ eqm_train_group_kernel(const float* __restrict__ ref, const float* __restrict__ 
       if (overflow) scale = 0.f;
       nslots[tid] = 0;
       bad_cell[tid] = overflow ? 1 : 0;
+      if constexpr (NORM) {
+        if (c0 + tid < C) {
+          const float nc = norm[(int64_t)pass * C + c0 + tid];
+          if (!norm_monotone(kind, nc) ||
+              (mx > mn && !(mx - mn < INFINITY && norm_apply(mx, kind, nc) - norm_apply(mn, kind, nc) < INFINITY)))
+            bad_cell[tid] = 1;
+        }
+      }
       cell_n[tid] = (mx >= mn) ? 1 : 0;                // any valid value; the histogram total replaces it below
       cell_mn[tid] = mn;
       cell_scale[tid] = scale;
@@ -566,12 +597,19 @@ eqm_train_group_kernel(const float* __restrict__ ref, const float* __restrict__ 
       if (nn > 0) {
         if (cell_scale[cc] == 0.f) {
           qv = cell_mn[cc];  // every valid value equals mn (or the range is not finite: not supported, gives mn)
+          if constexpr (NORM) qv = norm_apply(qv, kind, norm[(int64_t)pass * C + c0 + cc]);
         } else if (!bad_cell[cc]) {
           const double q = (double)(float)(((double)j + 0.5) / (double)nq);
           const double pos = q * (double)(nn - 1);
           const double lo = floor(pos);
           const double gq = pos - lo;
-          const double a0 = (double)tgt_val[cc * ntg + 2 * j], a1 = (double)tgt_val[cc * ntg + 2 * j + 1];
+          float v0 = tgt_val[cc * ntg + 2 * j], v1 = tgt_val[cc * ntg + 2 * j + 1];
+          if constexpr (NORM) {
+            const float nc = norm[(int64_t)pass * C + c0 + cc];
+            v0 = norm_apply(v0, kind, nc);
+            v1 = norm_apply(v1, kind, nc);
+          }
+          const double a0 = (double)v0, a1 = (double)v1;
           const double d = a1 - a0;
           qv = (float)((gq >= 0.5) ? (a1 - d * (1.0 - gq)) : (a0 + d * gq));
         }
@@ -694,6 +732,23 @@ eqm_adjust_kernel(const float* __restrict__ sim, int64_t T, int64_t C, int64_t l
   }
 }
 
+// DQM train, before the selection: the one period [0, T) of the mean pass
+__global__ void dqm_poff_kernel(int32_t* __restrict__ poff, int32_t T) {
+  poff[0] = 0;
+  poff[1] = T;
+}
+
+// DQM train: m = the means [2][C] of ref and hist -> scaling = m_ref - m_hist ("+") or m_ref / m_hist ("*"), and in
+// place the normalisation constants inv(m) = -m ("+") or float32(1 / m) ("*")
+__global__ void dqm_norm_kernel(float* __restrict__ m, int64_t C, int32_t kind, float* __restrict__ scaling) {
+  const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const float mr = m[c], mh = m[C + c];
+  scaling[c] = (kind == 0) ? __fsub_rn(mr, mh) : __fdiv_rn(mr, mh);
+  m[c] = (kind == 0) ? -mr : __fdiv_rn(1.f, mr);
+  m[C + c] = (kind == 0) ? -mh : __fdiv_rn(1.f, mh);
+}
+
 }  // namespace
 }  // namespace xc
 
@@ -705,48 +760,58 @@ extern "C" int64_t xc_eqm_train_workspace_bytes(int64_t T, int64_t C, int32_t nq
   return 256 + (2 * C + 1) * 4;
 }
 
-// the one-cell-per-CTA kernel on `grid` CTAs: every cell (redo == nullptr, grid == C) or a work list
+// the one-cell-per-CTA kernel on `grid` CTAs: every cell (redo == nullptr, grid == C) or a work list; with `norm`
+// (DQM) the NORM instantiation
 static int32_t launch_train_cells(const float* ref, const float* hist, int64_t T, int64_t C, int64_t ldx, int32_t nq,
                                   int32_t kind, float* af, float* hist_q, const int32_t* redo, unsigned grid,
-                                  cudaStream_t st) {
+                                  const float* norm, cudaStream_t st) {
   int npad = 1024;
   while (npad < T) npad <<= 1;
   const size_t smem = ((size_t)npad + ((nq + 3) & ~3) + (size_t)2 * nq * kCap) * 4;
+  auto go = [&](auto NORMC) -> int32_t {
+    constexpr bool NORM = decltype(NORMC)::value;
 #define XC_TRAIN(NP)                                                                                               \
   do {                                                                                                             \
     if (smem > 48 * 1024) {                                                                                        \
-      cudaError_t e_ = cudaFuncSetAttribute(eqm_train_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
+      cudaError_t e_ = cudaFuncSetAttribute(eqm_train_kernel<NP, NORM>, cudaFuncAttributeMaxDynamicSharedMemorySize,\
                                             (int)smem);                                                            \
       if (e_ != cudaSuccess) return cuda_fail(e_, "cudaFuncSetAttribute(eqm_train_kernel)");                       \
     }                                                                                                              \
-    eqm_train_kernel<NP><<<grid, kSortThreads, smem, st>>>(ref, hist, (int32_t)T, C, ldx, nq, kind, af, hist_q,    \
-                                                           redo);                                                  \
+    eqm_train_kernel<NP, NORM><<<grid, kSortThreads, smem, st>>>(ref, hist, (int32_t)T, C, ldx, nq, kind, af,      \
+                                                                 hist_q, redo, norm);                              \
   } while (0)
-  switch (npad) {
-    case 1024: XC_TRAIN(1024); break;
-    case 2048: XC_TRAIN(2048); break;
-    case 4096: XC_TRAIN(4096); break;
-    case 8192: XC_TRAIN(8192); break;
-    case 16384: XC_TRAIN(16384); break;
-    default: XC_TRAIN(32768); break;
-  }
+    switch (npad) {
+      case 1024: XC_TRAIN(1024); break;
+      case 2048: XC_TRAIN(2048); break;
+      case 4096: XC_TRAIN(4096); break;
+      case 8192: XC_TRAIN(8192); break;
+      case 16384: XC_TRAIN(16384); break;
+      default: XC_TRAIN(32768); break;
+    }
 #undef XC_TRAIN
-  return launch_status("eqm_train_kernel");
+    return launch_status("eqm_train_kernel");
+  };
+  return norm ? go(std::true_type{}) : go(std::false_type{});
 }
 
-extern "C" int32_t xc_eqm_train_f32(const float* ref, const float* hist, int64_t T, int64_t C, int64_t ldx,
-                                    int32_t nq, int32_t kind, float* af, float* hist_q, void* workspace,
-                                    int64_t workspace_bytes, void* stream) {
+static int32_t check_train_args(const float* ref, const float* hist, int64_t T, int64_t C, int64_t ldx, int32_t nq,
+                                int32_t kind, const float* af, const float* hist_q, const char* who) {
   XC_REQUIRE(ref && hist && af && hist_q, "null pointer argument");
   XC_REQUIRE(T > 0 && C > 0 && ldx >= C, "bad shape");
   XC_REQUIRE(nq >= 1 && nq <= 64, "nquantiles must be in [1, 64]");
   XC_REQUIRE(kind == 0 || kind == 1, "kind must be 0 ('+') or 1 ('*')");
   XC_REQUIRE(C <= 2147483647LL, "too many cells for one launch");
   if (T > 32768) {
-    set_error("eqm_train: series longer than 32768 steps do not fit the shared-memory sort");
+    set_error("%s: series longer than 32768 steps do not fit the shared-memory sort", who);
     return XC_ERR_UNSUPPORTED;
   }
-  cudaStream_t st = (cudaStream_t)stream;
+  return XC_OK;
+}
+
+// EQM train (norm == nullptr) or DQM train on the normalised series (norm: [2][C] device, see norm_apply)
+static int32_t train_impl(const float* ref, const float* hist, int64_t T, int64_t C, int64_t ldx, int32_t nq,
+                          int32_t kind, float* af, float* hist_q, void* workspace, int64_t workspace_bytes,
+                          const float* norm, cudaStream_t st) {
   const int64_t need = xc_eqm_train_workspace_bytes(T, C, nq);
   // widest group first: 32 cells = 128 bytes per (CTA, time row) touch; 16 when C is not a multiple of 32 or the
   // targets of 32 cells do not fit in shared memory.  (A variant that staged a 4-cell slice in shared memory and
@@ -761,27 +826,39 @@ extern "C" int32_t xc_eqm_train_f32(const float* ref, const float* hist, int64_t
   if (workspace == nullptr || workspace_bytes < need || !vec_ok || !fits || getenv("XCLIM_B200_EQM_V1")) {
     // no scratch for a redo list, or a layout without whole 16-byte pieces per CTA: the one-cell-per-CTA
     // kernel (complete in itself)
-    return launch_train_cells(ref, hist, T, C, ldx, nq, kind, af, hist_q, nullptr, (unsigned)C, st);
+    return launch_train_cells(ref, hist, T, C, ldx, nq, kind, af, hist_q, nullptr, (unsigned)C, norm, st);
   }
   int32_t* redo = (int32_t*)workspace;
   XC_CHECK_CUDA(cudaMemsetAsync(redo, 0, 4, st));
   const size_t smemg = train_group_smem_bytes(g, 2 * nq);
   const int64_t groups = C / g;
+  auto go = [&](auto NORMC) -> int32_t {
+    constexpr bool NORM = decltype(NORMC)::value;
 #define XC_TRAIN_GROUP(G, GT)                                                                                      \
   do {                                                                                                             \
-    XC_CHECK_CUDA(cudaFuncSetAttribute(eqm_train_group_kernel<G, GT>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                       (int)smemg));                                                               \
-    eqm_train_group_kernel<G, GT><<<(unsigned)groups, GT, smemg, st>>>(ref, hist, (int32_t)T, C, ldx, nq, kind,   \
-                                                                        af, hist_q, redo);                         \
+    XC_CHECK_CUDA(cudaFuncSetAttribute(eqm_train_group_kernel<G, GT, NORM>,                                        \
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemg));                  \
+    eqm_train_group_kernel<G, GT, NORM><<<(unsigned)groups, GT, smemg, st>>>(ref, hist, (int32_t)T, C, ldx, nq,    \
+                                                                              kind, af, hist_q, redo, norm);       \
   } while (0)
-  if (g == 32 && gt_env && atoi(gt_env) == 512) XC_TRAIN_GROUP(32, 512);
-  else if (g == 32) XC_TRAIN_GROUP(32, 1024);
-  else XC_TRAIN_GROUP(16, 512);
+    if (g == 32 && gt_env && atoi(gt_env) == 512) XC_TRAIN_GROUP(32, 512);
+    else if (g == 32) XC_TRAIN_GROUP(32, 1024);
+    else XC_TRAIN_GROUP(16, 512);
 #undef XC_TRAIN_GROUP
-  int32_t e = launch_status("eqm_train_group_kernel");
+    return launch_status("eqm_train_group_kernel");
+  };
+  int32_t e = norm ? go(std::true_type{}) : go(std::false_type{});
   if (e) return e;
   // cells the eight-cell layout could not finish (heavy non-constant bins): a small fixed grid walks the list
-  return launch_train_cells(ref, hist, T, C, ldx, nq, kind, af, hist_q, redo, 2u * (unsigned)sm_count(), st);
+  return launch_train_cells(ref, hist, T, C, ldx, nq, kind, af, hist_q, redo, 2u * (unsigned)sm_count(), norm, st);
+}
+
+extern "C" int32_t xc_eqm_train_f32(const float* ref, const float* hist, int64_t T, int64_t C, int64_t ldx,
+                                    int32_t nq, int32_t kind, float* af, float* hist_q, void* workspace,
+                                    int64_t workspace_bytes, void* stream) {
+  if (int32_t e = check_train_args(ref, hist, T, C, ldx, nq, kind, af, hist_q, "eqm_train")) return e;
+  return train_impl(ref, hist, T, C, ldx, nq, kind, af, hist_q, workspace, workspace_bytes, nullptr,
+                    (cudaStream_t)stream);
 }
 
 extern "C" int32_t xc_eqm_adjust_f32(const float* sim, int64_t T, int64_t C, int64_t ldx, const float* af,
@@ -816,4 +893,39 @@ extern "C" int32_t xc_eqm_adjust_f32(const float* sim, int64_t T, int64_t C, int
   else XC_ADJ(1, 1);
 #undef XC_ADJ
   return launch_status("eqm_adjust_kernel");
+}
+
+// workspace of xc_dqm_train_f32: the period offsets | the means, then normalisation constants [2][C] | EQM's
+static int64_t dqm_means_bytes(int64_t C) { return (8 * C + 255) / 256 * 256; }
+
+extern "C" int64_t xc_dqm_train_workspace_bytes(int64_t T, int64_t C, int32_t nq) {
+  C = C < 1 ? 1 : C;
+  return 256 + dqm_means_bytes(C) + xc_eqm_train_workspace_bytes(T, C, nq);
+}
+
+extern "C" int32_t xc_dqm_train_f32(const float* ref, const float* hist, int64_t T, int64_t C, int64_t ldx,
+                                    int32_t nq, int32_t kind, float* af, float* hist_q, float* scaling,
+                                    void* workspace, int64_t workspace_bytes, void* stream) {
+  if (int32_t e = check_train_args(ref, hist, T, C, ldx, nq, kind, af, hist_q, "dqm_train")) return e;
+  XC_REQUIRE(scaling && workspace, "null pointer argument");
+  const int64_t need = xc_dqm_train_workspace_bytes(T, C, nq);
+  XC_REQUIRE(workspace_bytes >= need, "workspace too small: %lld bytes, at least %lld needed",
+             (long long)workspace_bytes, (long long)need);
+  cudaStream_t st = (cudaStream_t)stream;
+  char* base = reinterpret_cast<char*>(workspace);
+  int32_t* poff = reinterpret_cast<int32_t*>(base);
+  float* m = reinterpret_cast<float*>(base + 256);
+  const int64_t used = 256 + dqm_means_bytes(C);
+  dqm_poff_kernel<<<1, 1, 0, st>>>(poff, (int32_t)T);
+  if (int32_t e = launch_status("dqm_poff_kernel")) return e;
+  // the NaN-skipping means: float64 sums of the valid values over n, rounded once (the tg_mean pass, P = 1)
+  if (int32_t e = xc_period_reduce_f32(ref, T, C, ldx, poff, 1, XC_STAT_MEAN, XC_TF_NONE, XC_OP_GT, 0.0, m, nullptr,
+                                       stream))
+    return e;
+  if (int32_t e = xc_period_reduce_f32(hist, T, C, ldx, poff, 1, XC_STAT_MEAN, XC_TF_NONE, XC_OP_GT, 0.0, m + C,
+                                       nullptr, stream))
+    return e;
+  dqm_norm_kernel<<<(unsigned)((C + 255) / 256), 256, 0, st>>>(m, C, kind, scaling);
+  if (int32_t e = launch_status("dqm_norm_kernel")) return e;
+  return train_impl(ref, hist, T, C, ldx, nq, kind, af, hist_q, base + used, workspace_bytes - used, m, st);
 }

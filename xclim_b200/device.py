@@ -373,6 +373,61 @@ def qdm_adjust(sim2d, af, nodes, kind_code, interp_code, want_sim_q=False, works
     return scen, sim_q
 
 
+def dqm_train(ref2d, hist2d, nq, kind_code):
+    """Detrended quantile mapping train (xc_dqm_train_f32): ``(af, hist_q, scaling)``, af / hist_q (nq, C) and
+    scaling (C,) float32 -- EQM's quantiles of the mean-normalised ref and hist, and the ratio of their means."""
+    T, C = ref2d.shape
+    assert hist2d.shape == ref2d.shape and ref2d.stride(0) == hist2d.stride(0)
+    af = torch.empty((nq, C), dtype=torch.float32, device=ref2d.device)
+    hq = torch.empty((nq, C), dtype=torch.float32, device=ref2d.device)
+    scaling = torch.empty(C, dtype=torch.float32, device=ref2d.device)
+    lib = load()
+    ws = torch.empty(int(lib.xc_dqm_train_workspace_bytes(T, C, int(nq))), dtype=torch.uint8, device=ref2d.device)
+    check(lib.xc_dqm_train_f32(ref2d.data_ptr(), hist2d.data_ptr(), T, C, ref2d.stride(0), int(nq), kind_code,
+                               af.data_ptr(), hq.data_ptr(), scaling.data_ptr(), ws.data_ptr(), ws.numel(),
+                               current_stream_ptr()))
+    return af, hq, scaling
+
+
+def poly_fit(x2d, degree, kind_code=0, scaling=None):
+    """Per-cell least-squares polynomial of ``degree`` over the valid steps (xc_poly_fit_f32): (degree + 1, C)
+    float64 coefficients in the basis u_t = (2t - (T - 1)) / max(T - 1, 1).  With ``scaling`` ((C,) float32) the
+    series fitted is float32(x + scaling) (kind 0) or float32(x * scaling) (kind 1)."""
+    T, C = x2d.shape
+    coef = torch.empty((int(degree) + 1, C), dtype=torch.float64, device=x2d.device)
+    if scaling is not None:
+        assert scaling.dtype == torch.float32 and scaling.is_contiguous() and scaling.numel() == C
+    check(load().xc_poly_fit_f32(x2d.data_ptr(), T, C, x2d.stride(0), int(degree), kind_code, _ptr(scaling),
+                                 coef.data_ptr(), current_stream_ptr()))
+    return coef
+
+
+def dqm_adjust(sim2d, af, hq, scaling, kind_code, interp_code, degree, want_coef=False):
+    """Detrended quantile mapping adjust: the trend of float32(sim (+|*) scaling) (poly_fit), then one streaming pass
+    (xc_dqm_adjust_f32).  Returns ``scen`` (T, C) float32, or ``(scen, coef)`` with ``want_coef``."""
+    T, C = sim2d.shape
+    nq = af.shape[0]
+    for t in (af, hq):
+        assert t.shape == (nq, C) and t.is_contiguous() and t.dtype == torch.float32
+    coef = poly_fit(sim2d, degree, kind_code, scaling)
+    scen = torch.empty((T, C), dtype=torch.float32, device=sim2d.device)
+    check(load().xc_dqm_adjust_f32(sim2d.data_ptr(), T, C, sim2d.stride(0), af.data_ptr(), hq.data_ptr(),
+                                   scaling.data_ptr(), coef.data_ptr(), nq, kind_code, interp_code, int(degree),
+                                   scen.data_ptr(), current_stream_ptr()))
+    return (scen, coef) if want_coef else scen
+
+
+def detrend(x2d, degree):
+    """``x - trend`` in float64 (T, C), the trend being the degree-``degree`` least-squares polynomial of x itself
+    over its valid steps (poly_fit, then xc_detrend_apply_f32)."""
+    T, C = x2d.shape
+    coef = poly_fit(x2d, degree)
+    out = torch.empty((T, C), dtype=torch.float64, device=x2d.device)
+    check(load().xc_detrend_apply_f32(x2d.data_ptr(), T, C, x2d.stride(0), coef.data_ptr(), int(degree),
+                                      out.data_ptr(), current_stream_ptr()))
+    return out
+
+
 def period_boundary_run(x2d, poff, op_code, thr, window, last=False, cmp_f64=False):
     """Index of the first (last) run of >= window steps per period, NaN if none (run_length.py:543-740)."""
     T, C = x2d.shape

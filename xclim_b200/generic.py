@@ -325,6 +325,30 @@ def count_level_crossings(low_data, high_data, threshold, freq, *, op_low="<", o
                                        var_reducer="all", constrain_var1=("<", "<="), constrain_var2=(">", ">="))
 
 
+# --------------------------------------------------------------------------------- detrend
+def detrend(ds, dim="time", deg=1):
+    """``ds`` minus its polynomial trend of degree ``deg`` along time -- indices/generic.py:1711-1736 (``polyfit``
+    then ``polyval``, ``ds - trend`` with the attributes kept).  The trend of each cell is the least-squares
+    polynomial over its valid steps (a gap-free daily axis); the result is float64, as float32 data minus the
+    float64 trend is in the reference, and NaN where ``ds`` is NaN.  DataArray / Field inputs, ``dim="time"`` and
+    degrees 0 to 2 only."""
+    from .field import Field
+    if not (isinstance(ds, Field) or is_xarray(ds)):
+        raise NotImplementedError(f"detrend takes a DataArray or a Field, got {type(ds).__name__}")
+    if dim != "time":
+        raise NotImplementedError("detrend along a dimension other than time is not supported")
+    if isinstance(deg, bool) or not isinstance(deg, (int, np.integer)) or deg < 0:
+        raise ValueError(f"deg must be a non-negative integer, got {deg!r}")
+    if deg > 2:
+        raise NotImplementedError(f"deg={deg}: only polynomial degrees 0, 1 and 2 are supported")
+    dims = dims_of(ds)
+    x2d, cell_shape, other, ta = _unwrap(ds)
+    out = device.detrend(x2d, int(deg))
+    vals = np.moveaxis(out.reshape((out.shape[0],) + cell_shape).cpu().numpy(), 0, dims.index("time"))
+    return wrap_like(ds, vals, dims, time=ta if ta.coord is None else ta.coord, attrs=attrs_of(ds),
+                     name=getattr(ds, "name", None))
+
+
 # --------------------------------------------------------------------------------- a12 seasons / dates
 def season(data, thresh, window, op, stat, freq, mid_date=None, constrain=None):
     """Season start / end (day of year) or length -- indices/generic.py:769-853 (+ run_length.py:891-1145)."""

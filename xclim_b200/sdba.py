@@ -1,10 +1,11 @@
-"""CUDA implementation behind ``xclim.sdba.EmpiricalQuantileMapping`` and ``QuantileDeltaMapping`` (xsdba;
-PARITY UNPINNED).
+"""CUDA implementation behind ``xclim.sdba.EmpiricalQuantileMapping``, ``QuantileDeltaMapping`` and
+``DetrendedQuantileMapping`` (xsdba; PARITY UNPINNED).
 
 ``xclim.sdba`` is a shim over the third-party ``xsdba`` package (sdba.py:11) whose sources are not
 part of the reference tree; the algorithm below follows its published behaviour and the reference's
 call sites (tests/test_xsdba.py:21-34, 143-150): ``EQM.train(ref, hist, nquantiles=, kind=,
-group="time")`` then ``.adjust(sim, interp=, extrapolation="constant")``; QDM trains the same way.
+group="time")`` then ``.adjust(sim, interp=, extrapolation="constant")``; QDM trains the same way, DQM on
+mean-normalised series.
 """
 from __future__ import annotations
 
@@ -35,6 +36,13 @@ class EmpiricalQuantileMapping:
 
     @classmethod
     def train(cls, ref, hist, *, nquantiles=20, kind="+", group="time", **kwargs):
+        r2, h2, cell_shape, other = cls._train_inputs(ref, hist, nquantiles, kind, group, kwargs)
+        af, hq = device.eqm_train(r2, h2, int(nquantiles), _KINDS[kind])
+        return cls(af, hq, int(nquantiles), kind, ref, cell_shape, other)
+
+    @staticmethod
+    def _train_inputs(ref, hist, nquantiles, kind, group, kwargs):
+        """Validate the train options and unwrap ref, hist to (T, C): ``(r2, h2, cell_shape, other_dims)``."""
         if group != "time":
             raise NotImplementedError("only group='time' is part of the xclim_b200 hot path")
         if kwargs:
@@ -47,8 +55,7 @@ class EmpiricalQuantileMapping:
         h2, cs2, _, _ = _unwrap(hist)
         if cs2 != cell_shape or h2.shape != r2.shape:
             raise ValueError("ref and hist must share the same shape")
-        af, hq = device.eqm_train(r2, h2, int(nquantiles), _KINDS[kind])
-        return cls(af, hq, int(nquantiles), kind, ref, cell_shape, other)
+        return r2, h2, cell_shape, other
 
     @property
     def ds(self):
@@ -104,3 +111,50 @@ class QuantileDeltaMapping(EmpiricalQuantileMapping):
         q = self._wrap_series(sim, sim_q, other, ta, "sim_q",
                               {"units": "", "long_name": "Percentage rank of sim within its series"})
         return {"scen": out, "sim_q": q}
+
+
+def _detrend_degree(detrend):
+    """xsdba's ``detrend`` argument of DQM / ``adjust``: an int is the degree of a PolyDetrend (``True`` / ``False``
+    are 1 / 0, as ``isinstance(detrend, int)`` accepts them); Detrend objects are not supported."""
+    if not isinstance(detrend, (int, np.integer)):
+        raise NotImplementedError(f"detrend={detrend!r}: only integer polynomial degrees 0, 1 and 2 are supported")
+    deg = int(detrend)
+    if not 0 <= deg <= 2:
+        raise NotImplementedError(f"detrend={deg}: only polynomial degrees 0, 1 and 2 are supported")
+    return deg
+
+
+class DetrendedQuantileMapping(EmpiricalQuantileMapping):
+    """Detrended quantile mapping bias adjustment, group="time" (xsdba ``DetrendedQuantileMapping``; PARITY UNPINNED).
+
+    ``train`` is EQM's on mean-normalised series: per cell, ``ref - mean(ref)`` and ``hist - mean(hist)`` ("+") or
+    ``ref * (1 / mean(ref))`` and ``hist * (1 / mean(hist))`` ("*"); ``.ds`` adds ``scaling``, the difference ("+")
+    or ratio ("*") of the two means.  ``adjust`` scales ``sim`` by ``scaling``, removes its polynomial trend of degree
+    ``detrend`` (fitted over the whole series of each cell), maps the detrended values through ``hist_q -> af`` and
+    puts the trend back, so that the trend of ``sim`` survives the correction.
+    """
+
+    def __init__(self, af, hist_q, scaling, nquantiles, kind, template, cell_shape, other_dims):
+        super().__init__(af, hist_q, nquantiles, kind, template, cell_shape, other_dims)
+        self._scaling = scaling                    # (C,) float32 device tensor
+
+    @classmethod
+    def train(cls, ref, hist, *, nquantiles=20, kind="+", group="time", **kwargs):
+        r2, h2, cell_shape, other = cls._train_inputs(ref, hist, nquantiles, kind, group, kwargs)
+        af, hq, scaling = device.dqm_train(r2, h2, int(nquantiles), _KINDS[kind])
+        return cls(af, hq, scaling, int(nquantiles), kind, ref, cell_shape, other)
+
+    @property
+    def ds(self):
+        """The trained dataset: ``af`` and ``hist_q`` (quantiles, *space) and ``scaling`` (*space)."""
+        out = super().ds
+        v = self._scaling.cpu().numpy().reshape(self._cell_shape)
+        out["scaling"] = wrap_like(self._template, v, self._other, attrs={"kind": self.kind, "group": "time"},
+                                   name="scaling")
+        return out
+
+    def adjust(self, sim, *, interp="nearest", extrapolation="constant", detrend=1, **kwargs):
+        deg = _detrend_degree(detrend)
+        s2, other, ta = self._unwrap_sim(sim, interp, extrapolation, kwargs)
+        scen = device.dqm_adjust(s2, self._af, self._hq, self._scaling, _KINDS[self.kind], _INTERP[interp], deg)
+        return self._wrap_series(sim, scen, other, ta, "scen", attrs_of(sim))
