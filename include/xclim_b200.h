@@ -468,7 +468,7 @@ int32_t xc_period_count_arr_f32(const float* x, int64_t T, int64_t C, int64_t ld
  *   plain:   sum / mean / min / max of x (select_resample_op, generic.py:83-125)
  *   Every `slot` is an index into `out` (slot s occupies out[s*P*C .. (s+1)*P*C), 4-byte elements: int32
  *   for n_true, float32 otherwise) or -1 when that output is not wanted.  n_runs is even.  Needs C % 4 == 0,
- *   ldx % 4 == 0 and 16-byte aligned buffers.
+ *   ldx % 4 == 0, 16-byte aligned buffers and T < 2^24 (counters and run lengths are float32).
  * ------------------------------------------------------------------------------------------- */
 #define XC_MULTI_MAX_COND 6
 #define XC_MULTI_MAX_RUNS 4

@@ -750,6 +750,9 @@ extern "C" int32_t xc_period_multi_f32(const float* x, int64_t T, int64_t C, int
   int32_t e = check_common(x, T, C, ldx, period_offsets, P, out);
   if (e) return e;
   XC_REQUIRE(plan_host != nullptr, "null pointer argument");
+  // run lengths and counters are float32: exact integers only below 2^24 steps
+  XC_REQUIRE(T < (1LL << 24), "xc_period_multi_f32 counts in float32: time axis must be shorter than 2^24 steps, got %lld",
+             (long long)T);
   XcMultiPlan pl = *plan_host;
   XC_REQUIRE(pl.n_cond >= 0 && pl.n_cond <= XC_MULTI_MAX_COND && pl.n_runs >= 0 && pl.n_runs <= XC_MULTI_MAX_RUNS &&
                  pl.n_runs % 2 == 0 && pl.n_msum >= 0 && pl.n_msum <= XC_MULTI_MAX_MSUM && pl.n_sums >= 0 &&

@@ -520,26 +520,37 @@ def period_run_quantile(x2d, poff, op_code, thr, q, window, resample_before_rl=T
 # ------------------------------------------------------------------------------------ fused multi-output pass
 def normalise_condition(op_code, thr):
     """(sgn, thr') with  x op thr  <=>  sgn * x > thr'  for every float32 x (NaN: False on both sides).
-    ``thr`` is compared in float32 (numpy >= 2 weak-scalar rule, indices/generic.py:301-326)."""
-    t = np.float32(thr)
+    ``thr`` is compared in float32 (numpy >= 2 weak-scalar rule, indices/generic.py:301-326).  Raises
+    NotImplementedError for the conditions no strict ``>`` expresses: ``x >= -inf`` and ``x <= +inf`` (true for
+    every non-NaN x, including the infinity itself, which has no float32 predecessor)."""
     gt, lt, ge, le = _lib.OPS[">"], _lib.OPS["<"], _lib.OPS[">="], _lib.OPS["<="]
-    if op_code == gt:
-        return 1.0, float(t)
-    if op_code == lt:
-        return -1.0, float(-t)
-    if op_code == ge:                      # x >= t  <=>  x > pred(t)
-        return 1.0, float(np.nextafter(t, np.float32(-np.inf)))
-    if op_code == le:                      # x <= t  <=>  -x >= -t  <=>  -x > pred(-t)
-        return -1.0, float(np.nextafter(np.float32(-t), np.float32(-np.inf)))
+    with np.errstate(over="ignore"):       # Python floats beyond float32 round to +-inf, as numpy compares them
+        t = np.float32(thr)
+        if op_code == gt:
+            return 1.0, float(t)
+        if op_code == lt:
+            return -1.0, float(-t)
+        if (op_code == ge and t == -np.inf) or (op_code == le and t == np.inf):
+            raise NotImplementedError(f"the fused pass cannot express x {'>=' if op_code == ge else '<='} {float(t)}")
+        if op_code == ge:                  # x >= t  <=>  x > pred(t)
+            return 1.0, float(np.nextafter(t, np.float32(-np.inf)))
+        if op_code == le:                  # x <= t  <=>  -x >= -t  <=>  -x > pred(-t)
+            return -1.0, float(np.nextafter(np.float32(-t), np.float32(-np.inf)))
     raise NotImplementedError("the fused pass takes the operators >, >=, <, <=")
 
 
 def period_multi(x2d, poff, plan, n_slots):
     """One streaming pass producing every output of ``plan`` (a ``_lib.MultiPlan``); returns the
-    ``(n_slots, P, C)`` float32 slot buffer (count slots hold int32 bits: view them with ``.view(torch.int32)``)."""
+    ``(n_slots, P, C)`` float32 slot buffer (count slots hold int32 bits: view them with ``.view(torch.int32)``).
+    The kernel reads four cells per 16-byte load; a grid whose cell count or row stride is not a multiple of 4
+    (small regional grids) is copied once into a zero-padded buffer that is."""
     import ctypes
     T, C = x2d.shape
     P = len(poff) - 1
+    if C % 4 or x2d.stride(0) % 4 or x2d.stride(1) != 1 or x2d.data_ptr() % 16:
+        xp = torch.zeros((T, (C + 3) // 4 * 4), dtype=torch.float32, device=x2d.device)
+        xp[:, :C] = x2d
+        return period_multi(xp, poff, plan, n_slots)[:, :, :C].contiguous()
     poff_d = dev_ints(poff, np.int32, x2d.device)
     out = torch.empty((max(1, n_slots), P, C), dtype=torch.float32, device=x2d.device)
     check(load().xc_period_multi_f32(x2d.data_ptr(), T, C, x2d.stride(0), poff_d.data_ptr(), P, ctypes.byref(plan),

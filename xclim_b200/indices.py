@@ -769,7 +769,8 @@ class _PassBuilder:
     def plans(self):
         """-> list of (plan, n_slots, {request key: (slot, is_int)}).  Layout of a plan (include/xclim_b200.h):
         the conditions that own run outputs come first, two output places each (a condition with more than two
-        is listed again), the one with a largest-run-sum output is condition 0."""
+        is listed again), the one with a largest-run-sum output is condition 0.  A largest-run-sum owner without
+        run outputs still takes run place 0 when other conditions own runs, so that it leaves room for one."""
         from . import _lib
         # units: one entry per condition place = (key, cond dict, [run outputs (<= 2)], wants n/max here?)
         places = []
@@ -809,7 +810,7 @@ class _PassBuilder:
                     rest.append(pl)
                     continue
                 take.append(pl)
-                n_run_places += owns_runs
+                n_run_places += owns_runs or owns_ms        # a max-sum owner holds run place 0 either way
                 have_ms = have_ms or owns_ms
             # order: max-sum owner, then run owners, then the plain ones
             take.sort(key=lambda pl: (not (pl["first"] and pl["c"]["ms"] is not None), not pl["runs"]))
@@ -901,40 +902,46 @@ def run_batch(fields, pers=None, names=None):
                 results[nm] = fn(fields[var])
                 continue
             kind, spec = "stat", ("stat",) + tuple(spec[1:])
-        if kind == "stat":
-            pb.stats[spec[1]] = True
-            keys = ("stat", spec[1])
-        elif kind in ("count", "prop"):
-            c, k = pb.cond(_lib.OPS[op], thr)
-            c["n"] = True
-            keys = ("n",) + k
-        elif kind == "excess":
-            sgn = 1.0 if op in (">", ">=") else -1.0
-            key = (0, 0.0, 0.0, sgn, float(np.float32(thr)))
-            pb.sums[key] = True
-            keys = ("qsum",) + key
-        elif kind == "intensity":
-            c, k = pb.cond(_lib.OPS[op], thr)
-            c["n"] = True
-            key = (1, k[0], k[1], 0.0, 0.0)
-            pb.sums[key] = True
-            keys = (("qsum",) + key, ("n",) + k)
-        elif kind == "spell":
-            c, k = pb.cond(_lib.OPS[op], thr)
-            c["runs"].add((spec[1], int(par["window"])))
-            keys = (spec[1],) + k + (int(par["window"]),)
-        elif kind == "maxlen":
-            c, k = pb.cond(_lib.OPS[op], thr)
-            c["max"] = True
-            keys = ("max",) + k
-        elif kind == "maxsum":
-            c, k = pb.cond(_lib.OPS[">"], thr)
-            c["ms"] = (int(par["window"]), 1.0, float(np.float32(thr)))
-            keys = ("ms",) + k + (int(par["window"]),)
+        try:
+            if kind == "stat":
+                pb.stats[spec[1]] = True
+                keys = ("stat", spec[1])
+            elif kind in ("count", "prop"):
+                c, k = pb.cond(_lib.OPS[op], thr)
+                c["n"] = True
+                keys = ("n",) + k
+            elif kind == "excess":
+                sgn = 1.0 if op in (">", ">=") else -1.0
+                key = (0, 0.0, 0.0, sgn, float(np.float32(thr)))
+                pb.sums[key] = True
+                keys = ("qsum",) + key
+            elif kind == "intensity":
+                c, k = pb.cond(_lib.OPS[op], thr)
+                c["n"] = True
+                key = (1, k[0], k[1], 0.0, 0.0)
+                pb.sums[key] = True
+                keys = (("qsum",) + key, ("n",) + k)
+            elif kind == "spell":
+                c, k = pb.cond(_lib.OPS[op], thr)
+                c["runs"].add((spec[1], int(par["window"])))
+                keys = (spec[1],) + k + (int(par["window"]),)
+            elif kind == "maxlen":
+                c, k = pb.cond(_lib.OPS[op], thr)
+                c["max"] = True
+                keys = ("max",) + k
+            elif kind == "maxsum":
+                c, k = pb.cond(_lib.OPS[">"], thr)
+                c["ms"] = (int(par["window"]), 1.0, float(np.float32(thr)))
+                keys = ("ms",) + k + (int(par["window"]),)
+        except NotImplementedError:     # a condition the fused pass cannot express (device.normalise_condition)
+            results[nm] = fn(fields[var])
+            continue
         todo.append((nm, var, freq, spec, par, keys))
     # ---- one launch (or a few) per (variable, frequency)
     slots = {}           # (var, freq, request key) -> device tensor (P, C)
     for (var, freq), pb in passes.items():
+        if not (pb.stats or pb.conds or pb.sums):
+            continue
         x2d, cell_shape, other, ta = unwrapped[var]
         poff = ta.period_offsets(freq)
         for plan, n, where in pb.plans():
