@@ -251,6 +251,62 @@ def main():
         report("dqm_adjust linear nq=20 detrend=1 (trend fit + apply, sim -> scen)", ms, 3 * T * C * 4,
                {"fit_ms": ms_fit},
                cpu=lambda: DO.dqm_adjust(host["hist"], daf, dhq, dsc, "+", "linear", detrend=1))
+    if want("spi") and a.only:      # standardized precipitation index: opt-in (--only spi)
+        from xclim_b200.timeaxis import TimeAxis
+        ta = TimeAxis.daily("1981-01-01", T, "noleap")
+        pm = ta.period_offsets("MS")
+        Pm = pm.size - 1
+        gid = (ta.month[pm[:-1]] - 1).astype(np.int64)
+        order = np.argsort(gid, kind="stable")
+        goff = np.concatenate([[0], np.cumsum(np.bincount(gid, minlength=12))])
+        m, _ = device.period_reduce(pr, pm, _lib.STATS["mean"])
+        r = device.rolling_mean(m, 3)
+        prm, nz, nn, status = device.si_fit(r, goff, order, 0, 1, True, 0.0)
+        ms_res = timeit(lambda: device.period_reduce(pr, pm, _lib.STATS["mean"]), a.steps)
+        ms_roll = timeit(lambda: device.rolling_mean(m, 3), a.steps)
+        ms_fit = timeit(lambda: device.si_fit(r, goff, order, 0, 1, True, 0.0), a.steps)
+        ms_app = timeit(lambda: device.si_apply(r, gid, prm, nz, nn, 0), a.steps)
+        # sampled cells, the last ones included: the kernel's parameters against the oracle's fit (kernel log rule)
+        # and the kernel's index against the oracle's scipy transform of those parameters
+        from oracle import stdindex_oracle as SO
+        cols = np.unique(np.r_[np.linspace(0, C - 1, 48).astype(int), np.arange(C - 16, C)])
+        rs, ps = r[:, cols].cpu().numpy(), prm[:, :, cols].cpu().numpy()
+        po, _, _ = SO.fit_groups(rs, gid, 12, slice(None), "gamma", "ML", True, 0.0, numpy_logs=False)
+        si = device.si_apply(r, gid, prm, nz, nn, 0)[:, cols].cpu().numpy()
+        sio = SO.transform(rs, gid, ps, "gamma", nz[:, cols].cpu().numpy(), nn[:, cols].cpu().numpy())
+        ok = ~np.isnan(sio)
+        from scipy.stats import norm
+        import subprocess
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True)
+        card = {"gpu": torch.cuda.get_device_name(), "power_limit": q.stdout.strip() or "unknown"}
+        check = {"cells": int(cols.size), "status": status, "nan_pattern_equal": bool(np.array_equal(np.isnan(si), ~ok)),
+                 "max_shape_rel_diff": float(np.nanmax(np.abs(ps[:, 0] - po[:, 0]) / np.abs(po[:, 0]))),
+                 "max_dsi_times_pdf": float(np.max(np.abs(si - sio)[ok] * norm.pdf(sio[ok])))}
+        report("spi monthly SPI-3 gamma ML floc=0: resample + rolling + fit + apply", ms_res + ms_roll + ms_fit + ms_app,
+               T * C * 4 + Pm * C * 4 + Pm * C * 4 + Pm * C * 8,
+               {"resample_ms": ms_res, "resample_algorithmic_bytes": T * C * 4 + Pm * C * 4,
+                "resample_gbs": (T * C * 4 + Pm * C * 4) / (ms_res * 1e-3) / 1e9, "rolling_ms": ms_roll,
+                "fit_ms": ms_fit, "apply_ms": ms_app, "apply_elements_per_s": Pm * C / (ms_app * 1e-3),
+                "apply_bound": "FP64 pipe: P(a, x) by series / continued fraction (tens of iterations) and two Halley "
+                               "steps of the inverse normal per element",
+                "check": check, **card})
+        del m, r, prm, nz, nn
+        Cd = min(a.lat, 90) * X                   # daily SPI-30 on a band: its float64 output is T * Cd * 8 bytes
+        prd = pr[:, :Cd]
+        gd = (ta.doy - 1).astype(np.int64)
+        od = np.argsort(gd, kind="stable")
+        gofd = np.concatenate([[0], np.cumsum(np.bincount(gd, minlength=365))])
+        rd = device.rolling_mean(prd, 30)
+        pd_, nzd, nnd, _ = device.si_fit(rd, gofd, od, 0, 1, True, 0.0)
+        ms_roll = timeit(lambda: device.rolling_mean(prd, 30), a.steps)
+        ms_fit = timeit(lambda: device.si_fit(rd, gofd, od, 0, 1, True, 0.0), a.steps)
+        ms_app = timeit(lambda: device.si_apply(rd, gd, pd_, nzd, nnd, 0), a.steps)
+        report(f"spi daily SPI-30 gamma ML floc=0 on {Cd // X} rows: rolling + fit + apply", ms_roll + ms_fit + ms_app,
+               T * Cd * 4 * 2 + T * Cd * 8,
+               {"rows": Cd // X, "rolling_ms": ms_roll, "fit_ms": ms_fit, "apply_ms": ms_app,
+                "apply_elements_per_s": T * Cd / (ms_app * 1e-3), **card})
+        del rd, pd_, nzd, nnd
     if want("fwi") and a.only:      # the fire-weather kernel: opt-in (--only fwi), never part of a default run
         import time
 

@@ -574,6 +574,51 @@ int32_t xc_fwi_f32(const float* tas, const float* pr, const float* hurs, const f
 int32_t xc_fwi_elementwise_f32(int32_t kind, const float* a, const float* b, int64_t n,
                                double p0, double p1, double p2, float* out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * s1  Standardized indices (SPI, SPEI) -- indices/stats.py
+ *   Replaces the rolling step of `preprocess_standardized_index` (:831-832), the per-(cell, group) fit of
+ *   `standardized_index_fit_params` (:944-953: `fit` -> `_fitfunc_1d` :45-112 -> `_fit_start` :576-684 and,
+ *   for ML, scipy's gamma_gen.fit / lognorm_gen.fit with a fixed loc) and the transform of
+ *   `standardized_index` (:1155-1191: rv_continuous.cdf, the zero-inflation algebra, norm.ppf, clip).
+ * ------------------------------------------------------------------------------------------- */
+/* out[t] = mean of x[t - window + 1 .. t] (float64 window sum, then float32(s / window)); NaN for the first
+ * window - 1 steps and for any window that holds a NaN: `rolling(time=window).mean(skipna=False)`.  out has
+ * leading dimension ldo (it may not alias x). */
+int32_t xc_rolling_mean_f32(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t window, float* out,
+                            int64_t ldo, void* stream);
+
+#define XC_SI_GAMMA   0
+#define XC_SI_FISK    1
+#define XC_SI_LOGNORM 2
+#define XC_SI_APP     0
+#define XC_SI_ML      1   /* with a fixed loc only (gamma, lognorm) */
+/* status word bits, OR-ed over all (cell, group) samples */
+#define XC_SI_STATUS_FITDATA          1   /* ML: a value <= floc (scipy FitDataError) */
+#define XC_SI_STATUS_ROOT_NAN         2   /* gamma ML: brentq met a NaN at a bracket end (constant samples) */
+#define XC_SI_STATUS_ROOT_SIGN        4   /* gamma ML: brentq bracket ends of one sign */
+#define XC_SI_STATUS_LOGNORM_FALLBACK 8   /* lognorm ML: zero spread; scipy runs its generic optimiser */
+
+/* Bytes of the fit workspace: one float32 per cell and value of the largest group (max_n values). */
+int64_t xc_si_fit_workspace_bytes(int64_t C, int32_t max_n);
+/* Fit every (group, cell): the sample of group g is x[steps[k], c] for k in [group_offsets[g],
+ * group_offsets[g+1]) (device int32 arrays, steps in time order), its finite values -- zeros left out when
+ * zero_inflated -- fitted with `dist` by `method` with loc fixed at floc.  Outputs (device): params (G, 3, C)
+ * float64 in scipy order (shape, loc, scale), NaN where the sample has <= 1 value or a parameter is NaN;
+ * n_zeros / n_notnull (G, C) int32 (values == 0, values not NaN; NULL when not zero_inflated); *status
+ * (device int32, OR-ed, caller zeroes it) gets XC_SI_STATUS_* bits.  max_n >= the largest group. */
+int32_t xc_si_fit_f32(const float* x, int64_t T, int64_t C, int64_t ldx, const int32_t* group_offsets,
+                      const int32_t* steps, int32_t G, int32_t max_n, int32_t dist, int32_t method,
+                      int32_t zero_inflated, double floc, double* params, int32_t* n_zeros, int32_t* n_notnull,
+                      int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
+/* out[t, c] (float64, leading dimension ldo) = the standardized index of x[t, c] under the parameters of
+ * group group_of_step[t] (device int16, -1 = NaN): params (G, 3, C) float64, counts (G, C) int32 (zero-inflated
+ * only, else NULL), interp = the zero-rank interpolation factor, (alpha, beta) = the zeros' plotting
+ * position. */
+int32_t xc_si_apply_f32(const float* x, int64_t T, int64_t C, int64_t ldx, const int16_t* group_of_step,
+                        int32_t G, const double* params, const int32_t* n_zeros, const int32_t* n_notnull,
+                        int32_t dist, int32_t zero_inflated, double interp, double alpha, double beta, double* out,
+                        int64_t ldo, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

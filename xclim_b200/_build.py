@@ -30,8 +30,9 @@ NVCC_FLAGS = [
 
 
 #: per-file flags.  fwi.cu mirrors numba / numpy arithmetic, which never fuses a multiply with an add; so does
-#: dqm.cu (the trend, detrend and retrend of the oracle, operation by operation).
-EXTRA_FLAGS = {"fwi.cu": ["-fmad=false"], "dqm.cu": ["-fmad=false"]}
+#: dqm.cu (the trend, detrend and retrend of the oracle, operation by operation) and stdindex.cu (numpy's float32
+#: moment expressions of the distribution fit).
+EXTRA_FLAGS = {"fwi.cu": ["-fmad=false"], "dqm.cu": ["-fmad=false"], "stdindex.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:

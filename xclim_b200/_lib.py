@@ -77,7 +77,18 @@ SIGNATURES = {
     "xc_fwi_elementwise_f32": (_i32, [_i32, _vp, _vp, _i64, _f64, _f64, _f64, _vp, _vp]),
     "xc_period_runstat_f32_host": (_i32, [_vp, _i64, _i64, _vp, _i32, _i32, _f64, _i32, _i32, _i32, _vp, _vp,
                                           _vp, _i64]),
+    "xc_rolling_mean_f32": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i64, _vp]),
+    "xc_si_fit_workspace_bytes": (_i64, [_i64, _i32]),
+    "xc_si_fit_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f64, _vp, _vp, _vp, _vp,
+                             _vp, _i64, _vp]),
+    "xc_si_apply_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _f64, _f64, _f64, _vp,
+                               _i64, _vp]),
 }
+
+# standardized indices (include/xclim_b200.h s1)
+SI_DISTS = {"gamma": 0, "fisk": 1, "lognorm": 2}
+SI_METHODS = {"APP": 0, "ML": 1}
+SI_STATUS_FITDATA, SI_STATUS_ROOT_NAN, SI_STATUS_ROOT_SIGN, SI_STATUS_LOGNORM_FALLBACK = 1, 2, 4, 8
 
 
 

@@ -15,6 +15,7 @@
 #include <type_traits>
 
 #include "../../include/xclim_b200.h"
+#include "npsum.cuh"
 
 #if defined(__CUDACC__)
 #define XC_FWI_HD __host__ __device__ __forceinline__
@@ -173,27 +174,13 @@ XC_FWI_HD float fwi_of(float isi, float bui) {                                  
 }
 XC_FWI_HD float dsr_of(float fwi) { return 0.0272f * powf(fwi, 1.77f); }              // :531-546
 
-// numpy's float32 mean of n <= 128 values (pairwise summation as np.add.reduce does it for one
-// contiguous run: plain loop below 8 values, else eight partial sums), oldest value first.
-// ring holds the last n values, the newest at index head.
+// numpy's float32 mean of n <= 128 values (one leaf of numpy's pairwise summation, npsum.cuh), oldest
+// value first.  ring holds the last n values, the newest at index head.
 XC_FWI_HD float np_mean_f32(const float* ring, int n, int head) {
   int i0 = head + 1;
   if (i0 >= n) i0 -= n;
   auto at = [&](int k) -> float { int j = i0 + k; if (j >= n) j -= n; return ring[j]; };
-  float res;
-  if (n < 8) {
-    res = 0.0f;
-    for (int k = 0; k < n; ++k) res += at(k);
-  } else {
-    float r[8];
-    for (int j = 0; j < 8; ++j) r[j] = at(j);
-    int k = 8;
-    for (; k < n - (n % 8); k += 8)
-      for (int j = 0; j < 8; ++j) r[j] += at(k + j);
-    res = ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7]));
-    for (; k < n; ++k) res += at(k);
-  }
-  return res / (float)n;
+  return np::pairwise_block_f32(at, n) / (float)n;
 }
 
 // ---- per-cell state -------------------------------------------------------------------------------

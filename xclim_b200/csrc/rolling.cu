@@ -862,10 +862,37 @@ rolling_period_reduce_sel_kernel(const float* __restrict__ x, int64_t T, int64_t
   out[(int64_t)p * C + c] = acc.result(stat);
 }
 
+// The rolled series itself (standardized indices, indices/stats.py:831-832): each label's window mean by
+// window_stat, a direct float64 sum of its w values, so an infinity stays confined to the windows holding it.
+// blockIdx.y walks chunks of kRollChunk labels; the window's other values are L1 / L2 hits.
+constexpr int kRollChunk = 32;
+
+__global__ void __launch_bounds__(kThreads)
+rolling_mean_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t ldx, int32_t w,
+                    float* __restrict__ out, int64_t ldo) {
+  const int64_t c = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+  if (c >= C) return;
+  const int t0 = blockIdx.y * kRollChunk;
+  const int t1 = min((int)T, t0 + kRollChunk);
+  for (int t = t0; t < t1; ++t)
+    out[(int64_t)t * ldo + c] = (t < w - 1) ? NAN : window_stat(x + c, ldx, t - w + 1, w, XC_STAT_MEAN);
+}
+
 }  // namespace
 }  // namespace xc
 
 using namespace xc;
+
+extern "C" int32_t xc_rolling_mean_f32(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t window, float* out,
+                                       int64_t ldo, void* stream) {
+  XC_REQUIRE(x && out, "null pointer argument");
+  XC_REQUIRE(T > 0 && C > 0 && ldx >= C && ldo >= C && T < 2147483647LL, "bad shape");
+  XC_REQUIRE(window >= 1, "window must be >= 1");
+  XC_REQUIRE((T + kRollChunk - 1) / kRollChunk <= 65535, "series longer than %d steps", 65535 * kRollChunk);
+  dim3 grid((unsigned)((C + kThreads - 1) / kThreads), (unsigned)((T + kRollChunk - 1) / kRollChunk), 1);
+  rolling_mean_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(x, T, C, ldx, window, out, ldo);
+  return launch_status("rolling_mean_kernel");
+}
 
 extern "C" int32_t xc_rolling_period_reduce_f32(const float* x, int64_t T, int64_t C, int64_t ldx,
                                                 const int32_t* period_offsets, int32_t P, int32_t window,

@@ -558,6 +558,57 @@ def period_multi(x2d, poff, plan, n_slots):
     return out
 
 
+# ------------------------------------------------------------------------------------ standardized indices
+def rolling_mean(x2d, window):
+    """``rolling(time=window).mean(skipna=False)`` as a new (T, C) float32 series (xc_rolling_mean_f32)."""
+    T, C = x2d.shape
+    out = torch.empty((T, C), dtype=torch.float32, device=x2d.device)
+    check(load().xc_rolling_mean_f32(x2d.data_ptr(), T, C, x2d.stride(0), int(window), out.data_ptr(), C,
+                                     current_stream_ptr()))
+    return out
+
+
+def si_fit(x2d, group_offsets, steps, dist_code, method_code, zero_inflated, floc):
+    """Fit every (group, cell) sample (xc_si_fit_f32).  ``group_offsets`` (G + 1) / ``steps``: host int arrays,
+    the CSR of each group's calibration steps.  Returns ``(params (G, 3, C) float64, n_zeros, n_notnull (G, C)
+    int32 or None, status int)``; reading the status synchronises the stream."""
+    T, C = x2d.shape
+    goff = np.ascontiguousarray(np.asarray(group_offsets, dtype=np.int32))
+    G = goff.size - 1
+    max_n = int(np.diff(goff).max()) if G > 0 else 0
+    st = np.ascontiguousarray(np.asarray(steps, dtype=np.int32))
+    goff_d = dev_ints(goff, np.int32, x2d.device)
+    steps_d = dev_ints(st if st.size else np.zeros(1, np.int32), np.int32, x2d.device)
+    lib = load()
+    ws = torch.empty(int(lib.xc_si_fit_workspace_bytes(C, max_n)), dtype=torch.uint8, device=x2d.device)
+    params = torch.empty((G, 3, C), dtype=torch.float64, device=x2d.device)
+    nz = torch.empty((G, C), dtype=torch.int32, device=x2d.device) if zero_inflated else None
+    nn = torch.empty((G, C), dtype=torch.int32, device=x2d.device) if zero_inflated else None
+    status = torch.zeros(1, dtype=torch.int32, device=x2d.device)
+    check(lib.xc_si_fit_f32(x2d.data_ptr(), T, C, x2d.stride(0), goff_d.data_ptr(), steps_d.data_ptr(), G, max_n,
+                            int(dist_code), int(method_code), int(bool(zero_inflated)), float(floc), params.data_ptr(),
+                            _ptr(nz), _ptr(nn), status.data_ptr(), ws.data_ptr(), ws.numel(), current_stream_ptr()))
+    return params, nz, nn, int(status.item())
+
+
+def si_apply(x2d, group_of_step, params, n_zeros, n_notnull, dist_code, interp=1.0, alpha=0.0, beta=1.0):
+    """(T, C) float64 standardized index (xc_si_apply_f32); ``group_of_step`` host int array, -1 = NaN;
+    ``n_zeros`` / ``n_notnull`` None for a distribution without zero inflation."""
+    T, C = x2d.shape
+    G = params.shape[0]
+    assert params.shape == (G, 3, C) and params.dtype == torch.float64 and params.is_contiguous()
+    zi = n_zeros is not None
+    if zi:
+        for t in (n_zeros, n_notnull):
+            assert t.shape == (G, C) and t.dtype == torch.int32 and t.is_contiguous()
+    gos = dev_ints(np.asarray(group_of_step, dtype=np.int16), np.int16, x2d.device)
+    out = torch.empty((T, C), dtype=torch.float64, device=x2d.device)
+    check(load().xc_si_apply_f32(x2d.data_ptr(), T, C, x2d.stride(0), gos.data_ptr(), G, params.data_ptr(),
+                                 _ptr(n_zeros), _ptr(n_notnull), int(dist_code), int(zi), float(interp), float(alpha),
+                                 float(beta), out.data_ptr(), C, current_stream_ptr()))
+    return out
+
+
 # ------------------------------------------------------------------------------------ fire weather
 FWI_OUTPUTS = ("DC", "DMC", "FFMC", "ISI", "BUI", "FWI", "DSR")
 

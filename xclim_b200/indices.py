@@ -1016,3 +1016,40 @@ def _stream_entry_points():
 
 
 _stream_entry_points()
+
+
+# ------------------------------------------------------------------ standardized indices (indices/_agro.py)
+_SI_DIST_METHODS = {"fisk": ["ML", "APP"], "gamma": ["ML", "APP"], "genextreme": ["ML"], "lognorm": ["ML", "APP"]}
+
+
+def _si_check(dist, method):
+    if isinstance(dist, str):
+        if dist in _SI_DIST_METHODS:
+            if method not in _SI_DIST_METHODS[dist]:
+                raise NotImplementedError(f"{method} method is not implemented for {dist} distribution")
+        else:
+            raise NotImplementedError(f"{dist} distribution is not yet implemented.")
+
+
+def standardized_precipitation_index(pr, freq="MS", window=1, dist="gamma", method="ML", fitkwargs=None,
+                                     cal_start=None, cal_end=None, params=None, prob_zero_interpolation="upper",
+                                     plotting_position_zero="ecdf", **indexer):
+    """Standardized Precipitation Index -- indices/_agro.py:987-1141 (zero-inflated)."""
+    from . import stats
+    fitkwargs = fitkwargs or {}
+    _si_check(dist, method)
+    return stats.standardized_index(pr, freq=freq, window=window, dist=dist, method=method, zero_inflated=True,
+                                    fitkwargs=fitkwargs, cal_start=cal_start, cal_end=cal_end, params=params,
+                                    prob_zero_interpolation=prob_zero_interpolation,
+                                    plotting_position_zero=plotting_position_zero, **indexer)
+
+
+def standardized_precipitation_evapotranspiration_index(wb, freq="MS", window=1, dist="gamma", method="ML",
+                                                        fitkwargs=None, cal_start=None, cal_end=None, params=None,
+                                                        **indexer):
+    """Standardized Precipitation Evapotranspiration Index -- indices/_agro.py:1148-1240 (not zero-inflated)."""
+    from . import stats
+    fitkwargs = fitkwargs or {}
+    _si_check(dist, method)
+    return stats.standardized_index(wb, freq=freq, window=window, dist=dist, method=method, zero_inflated=False,
+                                    fitkwargs=fitkwargs, cal_start=cal_start, cal_end=cal_end, params=params, **indexer)
