@@ -215,10 +215,13 @@ def rle(da, index="first"):
 # a10 rle_statistics / longest_run (indices/run_length.py:275-378)
 # --------------------------------------------------------------------------------------------------
 def _get_rl_stat(d, window, reducer):
-    """indices/run_length.py:320-327."""
+    """indices/run_length.py:320-327.  ``reducer`` may also be a float q in [0, 1]: the quantile q, as "qNN" is
+    the quantile 0.NN."""
     with np.errstate(all="ignore"), _quiet():
         dm = np.where(d >= window, d, np.nan)
-        if reducer.startswith("q") and reducer[1:].isdigit():
+        if isinstance(reducer, float):
+            stat = np.nanquantile(dm, reducer, axis=0)
+        elif reducer.startswith("q") and reducer[1:].isdigit():
             stat = np.nanquantile(dm, float(f"0.{reducer[1:]}"), axis=0)
         elif reducer == "count":
             stat = np.sum(~np.isnan(dm), axis=0).astype(np.float64)

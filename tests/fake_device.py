@@ -232,7 +232,7 @@ def eqm_adjust(sim2d, af, hq, kind_code, interp_code):
 
 def period_run_quantile(x2d, poff, op_code, thr, q, window, resample_before_rl=True, cmp_f64=False):
     out = O.resample_and_rl(_cond(_np(x2d), op_code, thr, cmp_f64), bool(resample_before_rl), O.rle_statistics,
-                            poff=poff, reducer=f"q{int(round(q * 100)):02d}", window=int(window))
+                            poff=poff, reducer=float(q), window=int(window))
     return torch.from_numpy(np.asarray(out, dtype=np.float32))
 
 

@@ -7,6 +7,9 @@ Outputs (committed):
   tests/golden/ref_run_length_1d.npz  -- statistics_run_1d / windowed_run_count_1d /
         windowed_run_events_1d / first_run_1d / _cumsum_reset_np on seeded boolean series
         (reference: indices/run_length.py:143-151, 1334-1477)
+  tests/golden/ref_run_quantile_1d.npz -- statistics_run_1d with the quantile reducers "qNN" and first_run_1d on
+        seeded boolean series and on one series with a run longer than 65535 steps
+        (reference: indices/run_length.py:1383-1437)
   tests/golden/ref_quantile.npz       -- calc_perc on seeded float32 samples with NaNs
         (reference: core/utils.py:279-557)
   tests/golden/ref_cffwis.npz         -- the fire-weather recurrences (_fire_weather_calc with its season,
@@ -68,6 +71,45 @@ def run_length_fixture(rng):
     np.savez_compressed(os.path.join(HERE, "ref_run_length_1d.npz"), series=series,
                         reducers=np.array(reducers), windows=np.array(windows), stats=stats,
                         wcount=wcount, wevents=wevents, first=first, cs_last=cs_last, cs_first=cs_first)
+
+
+#: reducers and windows of ref_run_quantile_1d.npz ("q5" is the quantile 0.5, "q05" 0.05, "q999" 0.999)
+RUN_QUANTILE_REDUCERS = ("q5", "q05", "q10", "q50", "q90", "q999")
+RUN_QUANTILE_WINDOWS = (1, 2, 5)
+
+
+def run_quantile_fixture():
+    """statistics_run_1d(arr, "qNN", w) and first_run_1d on seeded boolean series, plus one series holding a run of
+    70000 steps (longer than a 16-bit run length) between short runs."""
+    rl = ref.load_run_length()
+    rng = np.random.default_rng(20261016)
+    n_series, T = 40, 400
+    series = np.zeros((n_series, T), dtype=bool)
+    for i in range(n_series):
+        flips = rng.random(T) < rng.uniform(0.03, 0.6)
+        state, p = rng.random() < 0.5, rng.uniform(0.1, 0.9)
+        for t in range(T):
+            if flips[t]:
+                state = rng.random() < p
+            series[i, t] = state
+    series[0] = False
+    series[1] = True
+    series[2, ::2] = True                   # 200 runs of length 1
+    series[2, 1::2] = False
+    long = np.zeros(70040, dtype=bool)
+    long[3:8] = True
+    long[9:70009] = True
+    long[70011:70013] = True
+    long[70020:] = True
+    stats = np.array([[[float(rl["statistics_run_1d"](s, r, w)) for s in series] for w in RUN_QUANTILE_WINDOWS]
+                      for r in RUN_QUANTILE_REDUCERS])
+    first = np.array([[float(rl["first_run_1d"](s, w)) for s in series] for w in RUN_QUANTILE_WINDOWS])
+    long_stats = np.array([[float(rl["statistics_run_1d"](long, r, w)) for w in RUN_QUANTILE_WINDOWS]
+                           for r in RUN_QUANTILE_REDUCERS])
+    long_first = np.array([float(rl["first_run_1d"](long, w)) for w in RUN_QUANTILE_WINDOWS])
+    np.savez_compressed(os.path.join(HERE, "ref_run_quantile_1d.npz"), series=series, long=long,
+                        reducers=np.array(RUN_QUANTILE_REDUCERS), windows=np.array(RUN_QUANTILE_WINDOWS), stats=stats,
+                        first=first, long_stats=long_stats, long_first=long_first)
 
 
 def quantile_fixture(rng):
@@ -347,9 +389,13 @@ if __name__ == "__main__":
     if not ref.available():
         raise SystemExit("reference sources not found: set XCLIM_REFERENCE_ROOT to a checkout of xclim "
                          f"(now {ref.REF_ROOT!r})")
+    if sys.argv[1:] == ["run_quantile"]:          # the one fixture with its own seed: regenerated alone
+        run_quantile_fixture()
+        raise SystemExit(print("ref_run_quantile_1d.npz written to", HERE))
     rng = np.random.default_rng(20260923)
     run_length_fixture(rng)
     quantile_fixture(rng)
     cffwis_fixture()
     cross_check_fixture()
+    run_quantile_fixture()
     print("golden fixtures written to", HERE)

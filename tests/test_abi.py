@@ -98,6 +98,44 @@ def test_argument_validation_happens_before_any_device_work(lib):
     assert seen == [b""]
 
 
+def test_boundary_run_entry_points_validate_on_the_host(lib):
+    """xc_period_boundary_run_f32, xc_period_boundary_run_range_f32 and xc_period_run_quantile_f32 refuse null
+    pointers, P = 0, P > 65535, ldx < C, window 0, q outside [0, 1] and periods too long for the run list before any
+    device work."""
+    import ctypes as C
+    INVALID, UNSUPPORTED = -1, -2
+    buf = (C.c_float * 16)()
+    p = C.cast(buf, C.c_void_p)
+    offs = (C.c_int32 * 3)(0, 4, 8)
+    ip = C.cast(offs, C.c_void_p)
+
+    def run(x=p, T=8, Cn=4, ldx=4, poff=ip, P=2, window=1, out=p):
+        return lib.xc_period_boundary_run_f32(x, T, Cn, ldx, poff, P, 0, 0.0, 0, window, 0, out, None)
+
+    def rng_(x=p, T=8, Cn=4, ldx=4, poff=ip, lo=ip, hi=ip, P=2, window=1, out=p):
+        return lib.xc_period_boundary_run_range_f32(x, T, Cn, ldx, poff, lo, hi, P, 0, 0.0, 0, 0, window, 0, None,
+                                                    out, None)
+
+    def rq(x=p, T=8, Cn=4, ldx=4, poff=ip, ph=ip, P=2, q=0.5, window=1, out=p):
+        return lib.xc_period_run_quantile_f32(x, T, Cn, ldx, poff, ph, P, 0, 0.0, 0, q, window, 1, out, None)
+
+    for fn in (run, rng_, rq):
+        for kw in ({"x": None}, {"poff": None}, {"out": None}):
+            assert fn(**kw) == INVALID and b"null pointer" in lib.xc_last_error(), (fn.__name__, kw)
+        for kw in ({"P": 0}, {"P": 65536}, {"ldx": 3}, {"T": 0}):
+            assert fn(**kw) == INVALID and b"bad shape" in lib.xc_last_error(), (fn.__name__, kw)
+        assert fn(window=0) == INVALID and b"window" in lib.xc_last_error(), fn.__name__
+    assert rng_(lo=None) == INVALID and rng_(hi=None) == INVALID
+    assert rq(ph=None) == INVALID and b"null pointer" in lib.xc_last_error()
+    for q in (-1e-9, 1.0 + 1e-9, float("nan")):
+        assert rq(q=q) == INVALID and b"q in [0, 1]" in lib.xc_last_error(), q
+    # the run list is cap = len / 2 + 2 uint16 per lane, 128 lanes, at most 200 KiB of shared memory
+    first_rejected = next(L for L in range(1, 4000) if (L // 2 + 2) * 128 * 2 > 200 * 1024)
+    long = (C.c_int32 * 3)(0, 1, 1 + first_rejected)
+    assert rq(T=1 + first_rejected, ph=C.cast(long, C.c_void_p)) == UNSUPPORTED
+    assert f"periods of {first_rejected} steps".encode() in lib.xc_last_error()
+
+
 def test_fire_weather_argument_validation(lib):
     """xc_fwi_f32 / xc_fwi_elementwise_f32 refuse inconsistent arguments on the host, with the reference's
     message where it has one (indices/fire/_cffwis.py:1115-1117)."""

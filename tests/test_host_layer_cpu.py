@@ -210,6 +210,7 @@ GPU_BODIES = {
     "test_gpu_seasons": ["test_date_bounded_runs_parity", "test_growing_season_reference_known_answers",
                          "test_season_parity"],
     "test_gpu_boundary": ["test_first_last_run"],
+    "test_gpu_boundary_runs": ["test_public_run_indices", "test_public_season_indices"],
     "test_gpu_period_stats": ["test_bivariate_heat_waves", "test_cdd_reference_known_answers",
                               "test_hot_spell_max_magnitude", "test_resample_reductions",
                               "test_run_length_module_masks", "test_run_length_quantile_reducers",
@@ -255,6 +256,49 @@ def _gpu_body_cases():
 def test_gpu_test_bodies_over_oracle_backed_device(host, mod, name, kwargs):
     import importlib
     getattr(importlib.import_module(mod), name)(None, **kwargs)
+
+
+def test_stand_in_run_quantile_takes_q_exactly():
+    """The stand-in of xc_period_run_quantile_f32 computes the quantile q it is given: 0.999 is "q999" (not "q100",
+    the quantile 0.100), 0.05 is "q05", 0.5 is "q5"."""
+    import torch
+    rng = np.random.default_rng(999)
+    m = rng.random((400, 12)) < 0.7
+    poff = np.array([0, 31, 59, 200, 400], np.int32)
+    x = torch.from_numpy(m.astype(np.float32))
+    for before in (True, False):
+        for q, red in ((0.999, "q999"), (0.05, "q05"), (0.5, "q5"), (0.1, "q10")):
+            got = fake_device.period_run_quantile(x, poff, 0, 0.0, q, 1, before).numpy()
+            exp = O.resample_and_rl(m, before, O.rle_statistics, poff=poff, reducer=red, window=1)
+            np.testing.assert_array_equal(got, exp.astype(np.float32), err_msg=f"q={q} before={before}")
+        q100 = O.resample_and_rl(m, before, O.rle_statistics, poff=poff, reducer="q100", window=1)
+        assert not np.array_equal(fake_device.period_run_quantile(x, poff, 0, 0.0, 0.999, 1, before).numpy(),
+                                  q100.astype(np.float32))
+
+
+def test_scalar_threshold_compares_float64_scalars_in_float64():
+    """np.float64 (a subclass of Python float) and 0-d float64 arrays compare in float64, as numpy promotes them;
+    Python numbers and float32 scalars compare in float32 (NEP 50)."""
+    from xclim_b200.generic import _scalar_threshold
+    assert _scalar_threshold(np.float64(0.1)) == (0.1, True)
+    assert _scalar_threshold(np.array(0.1)) == (0.1, True)
+    assert _scalar_threshold(0.1) == (0.1, False)
+    assert _scalar_threshold(3) == (3.0, False)
+    assert _scalar_threshold(np.float32(0.5)) == (0.5, False)
+
+
+def test_first_occurrence_float64_threshold_over_stand_ins(host):
+    """first_occurrence with np.float64(278.15) on data holding float32(278.15): numpy compares in float64, where
+    that value is below the threshold."""
+    from xclim_b200 import generic
+    x = np.full((365, 2), 270.0, np.float32)
+    x[10, :] = np.float32(278.15)
+    x[20, 1] = 279.0
+    da = make_field(x, "2001-01-01", calendar="noleap", units="K")
+    got = generic.first_occurrence(da, np.float64(278.15), "YS", ">=").values
+    np.testing.assert_array_equal(got, [[np.nan, 21.0]])
+    got = generic.first_occurrence(da, 278.15, "YS", ">=").values
+    np.testing.assert_array_equal(got, [[11.0, 11.0]])
 
 
 def test_atmos_generic_missing_any_wrapper(host):

@@ -37,6 +37,29 @@ def test_run_length_whole_array_path_matches_reference_1d(golden_dir):
     np.testing.assert_array_equal(O.cumsum_reset(series, "first").T, g["cs_first"])
 
 
+def test_run_length_quantiles_match_reference_1d(golden_dir):
+    """O.rle_statistics with the "qNN" reducers (and with the same q as a float) and O.first_run at freq=None against
+    the reference's statistics_run_1d / first_run_1d, including one run of 70000 steps."""
+    g = np.load(os.path.join(golden_dir, "ref_run_quantile_1d.npz"))
+    series, long = g["series"].T, g["long"][:, None]
+    assert long.shape[0] > 65535 and g["long_stats"].max() > 65535
+    for ri, red in enumerate(g["reducers"]):
+        red = str(red)
+        q = float(f"0.{red[1:]}")
+        for wi, w in enumerate(g["windows"]):
+            for r in (red, q):
+                np.testing.assert_array_equal(O.rle_statistics(series, r, int(w)), g["stats"][ri, wi],
+                                              err_msg=f"{r} w={w}")
+                np.testing.assert_array_equal(O.rle_statistics(long, r, int(w))[0], g["long_stats"][ri, wi],
+                                              err_msg=f"{r} w={w} long")
+    for wi, w in enumerate(g["windows"]):
+        fr, exp = O.first_run(series, int(w)), g["first"][wi]
+        alltrue = series.all(axis=0) if int(w) == 1 else np.zeros(series.shape[1], bool)
+        np.testing.assert_array_equal(fr[~alltrue], exp[~alltrue])     # the whole-array argmax == argmin quirk
+        assert np.isnan(fr[alltrue]).all()
+        np.testing.assert_array_equal(O.first_run(long, int(w)), [g["long_first"][wi]])
+
+
 def test_quantile_matches_reference_calc_perc(golden_dir):
     g = np.load(os.path.join(golden_dir, "ref_quantile.npz"))
     pers = g["percentiles"]

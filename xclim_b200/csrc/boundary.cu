@@ -231,8 +231,11 @@ extern "C" int32_t xc_period_boundary_run_range_f32(const float* x, int64_t T, i
 // ------------------------------------------------------------------------------------------------
 // Replaces indices/run_length.py:320-327 with reducer = "quantile": `d.where(d >= window).quantile(q)`
 // (numpy's linear / type-7 quantile over the run lengths >= window attributed to the period; 0 when
-// there is none).  A lane owns one (period, cell): run lengths go to its shared-memory column
-// (uint16, at most ceil(len/2) runs), the two neighbouring order statistics are found by counting.
+// there is none).  A lane owns one (period, cell): the runs closed inside the period go to its
+// shared-memory column (uint16, at most ceil(len/2) runs, each at most len steps), the run still open
+// at the period end is held in a register (`tail`): with resample_before_rl=False it keeps its full
+// length up to the end of the series, which may exceed 65535.  The two neighbouring order statistics
+// are found by counting over both.
 namespace xc {
 namespace {
 
@@ -250,11 +253,10 @@ run_quantile_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t l
   int m = 0, cur = 0, longest = 0;
   bool skip = false;
   if (after && t0 > 0) skip = cmp<OP>(ld_stream(col + (int64_t)(t0 - 1) * ldx), thr);
-  auto close_run = [&]() {
+  auto close_run = [&]() {   // a run that ends inside the period: cur <= t1 - t0 < 65536
     if (cur >= window && m < cap) {
-      const int r = min(cur, 65535);
-      runs[(size_t)m++ * kThreads + lane] = (unsigned short)r;
-      longest = max(longest, r);
+      runs[(size_t)m++ * kThreads + lane] = (unsigned short)cur;
+      longest = max(longest, cur);
     }
     cur = 0;
   };
@@ -283,41 +285,40 @@ run_quantile_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t l
       pp += ldx;
     }
   }
-  if (after) {
-    int t = t1;
-    while (cur > 0 && t < (int)T) {
-      if (cmp<OP>(ld_stream(col + (int64_t)t * ldx), thr)) ++cur; else close_run();
-      ++t;
-    }
+  if (after) {   // the run open at t1 belongs to this period with its full length
+    for (int t = t1; cur > 0 && t < (int)T && cmp<OP>(ld_stream(col + (int64_t)t * ldx), thr); ++t) ++cur;
   }
-  close_run();
+  const int tail = cur >= window ? cur : 0;    // 0: no run
+  longest = max(longest, tail);
+  const int n = m + (tail > 0 ? 1 : 0);
   float res = 0.f;
-  if (m > 0) {
-    // numpy linear quantile: pos = q (m - 1); lerp of the two neighbouring order statistics
-    const double pos = q * (double)(m - 1);
+  if (n > 0) {
+    // numpy linear quantile: pos = q (n - 1); lerp of the two neighbouring order statistics
+    const double pos = q * (double)(n - 1);
     const int ilo = (int)floor(pos);
-    const int ihi = min(ilo + 1, m - 1);
+    const int ihi = min(ilo + 1, n - 1);
     const double g = pos - (double)ilo;
-    // order statistics ilo, ihi of m small integers: bisection on the VALUE (#{run <= v} is monotone in v), 16
-    // counting passes instead of the m^2 rank count; the upper neighbour is vlo itself when ties cover rank ihi,
-    // else the smallest length above vlo
+    // order statistics ilo, ihi of n integers: bisection on the VALUE (#{run <= v} is monotone in v), at most
+    // ceil(log2(longest + 1)) counting passes instead of the n^2 rank count; the upper neighbour is vlo itself when
+    // ties cover rank ihi, else the smallest length above vlo
     int lo_v = 0, hi_v = longest;              // smallest v with #{run <= v} >= ilo + 1
     while (lo_v < hi_v) {
-      const int mid = (lo_v + hi_v) >> 1;
-      int le = 0;
+      const int mid = lo_v + ((hi_v - lo_v) >> 1);
+      int le = (tail > 0 && tail <= mid) ? 1 : 0;
       for (int k = 0; k < m; ++k) le += (runs[(size_t)k * kThreads + lane] <= mid) ? 1 : 0;
       if (le >= ilo + 1) hi_v = mid; else lo_v = mid + 1;
     }
-    int le = 0, nxt = 65536;
+    int le = (tail > 0 && tail <= lo_v) ? 1 : 0;
+    int nxt = (tail > lo_v) ? tail : INT_MAX;
     for (int k = 0; k < m; ++k) {
       const int vk = runs[(size_t)k * kThreads + lane];
       le += (vk <= lo_v) ? 1 : 0;
       nxt = (vk > lo_v && vk < nxt) ? vk : nxt;
     }
-    const float vlo = (float)lo_v;
-    const float vhi = (le >= ihi + 1) ? vlo : (float)nxt;
-    const double d = (double)vhi - (double)vlo;
-    res = (float)((g >= 0.5) ? ((double)vhi - d * (1.0 - g)) : ((double)vlo + d * g));
+    const double vlo = (double)lo_v;
+    const double vhi = (le >= ihi + 1) ? vlo : (double)nxt;
+    const double d = vhi - vlo;
+    res = (float)((g >= 0.5) ? (vhi - d * (1.0 - g)) : (vlo + d * g));
   }
   out[(int64_t)p * C + c] = res;
 }

@@ -62,9 +62,10 @@ def _wrap_periods(da, out2d, cell_shape, other_dims, ta, freq, attrs, dtype=None
 
 def _scalar_threshold(threshold):
     """A Python number compares in float32 (numpy>=2 weak scalar); a 0-d float64 array/np.float64
-    compares in float64 (indices/generic.py:301-326 + NEP 50)."""
-    if isinstance(threshold, (np.floating,)) and threshold.dtype == np.float64 and not isinstance(threshold, float):
-        return float(threshold), True
+    compares in float64 (indices/generic.py:301-326 + NEP 50).  np.float64 subclasses float, so it is tested
+    first."""
+    if isinstance(threshold, np.floating):
+        return float(threshold), threshold.dtype == np.float64
     if isinstance(threshold, (int, float)):
         return float(threshold), False
     arr = np.asarray(getattr(threshold, "values", threshold))
