@@ -98,6 +98,43 @@ inline int32_t dispatch_op_nan(int32_t op, F&& f) {
   return dispatch_op(op, f);
 }
 
+// the shared-memory sort length of a series of T <= 32768 steps (the power of two >= T, at least 1024) as a
+// compile-time constant
+template <typename F>
+inline auto dispatch_npad(int64_t T, F&& f) {
+  if (T <= 1024) return f(std::integral_constant<int, 1024>{});
+  if (T <= 2048) return f(std::integral_constant<int, 2048>{});
+  if (T <= 4096) return f(std::integral_constant<int, 4096>{});
+  if (T <= 8192) return f(std::integral_constant<int, 8192>{});
+  if (T <= 16384) return f(std::integral_constant<int, 16384>{});
+  return f(std::integral_constant<int, 32768>{});
+}
+
+// interpolation (0 nearest, 1 linear) and kind (0 "+", 1 "*") of a quantile-mapping adjust as compile-time constants
+template <typename F>
+inline auto dispatch_interp_kind(int32_t interp, int32_t kind, F&& f) {
+  using I0 = std::integral_constant<int, 0>;
+  using I1 = std::integral_constant<int, 1>;
+  if (interp == 0) return kind == 0 ? f(I0{}, I0{}) : f(I0{}, I1{});
+  return kind == 0 ? f(I1{}, I0{}) : f(I1{}, I1{});
+}
+
+// nq in [nq_lo, nq_hi], kind and interp: the arguments every quantile-mapping entry point checks (train has no interp)
+inline int32_t check_qmap_args(int32_t nq, int nq_lo, int nq_hi, int32_t kind, int32_t interp = 0) {
+  XC_REQUIRE(nq >= nq_lo && nq <= nq_hi, "nquantiles must be in [%d, %d]", nq_lo, nq_hi);
+  XC_REQUIRE(kind == 0 || kind == 1, "kind must be 0 ('+') or 1 ('*')");
+  XC_REQUIRE(interp == 0 || interp == 1, "interp must be 0 (nearest) or 1 (linear)");
+  return XC_OK;
+}
+
+// lets `kernel` use `bytes` of dynamic shared memory (an opt-in above the default 48 KiB)
+template <typename Kernel>
+inline int32_t allow_smem(Kernel* kernel, size_t bytes, const char* what) {
+  if (bytes <= 48 * 1024) return XC_OK;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  return e == cudaSuccess ? XC_OK : cuda_fail(e, what);
+}
+
 // Block-wide bitonic sort of keys[0..NPAD) ascending in shared memory by NT threads (NaN-free keys): the
 // fallback sort of the EQM train and QDM rank kernels.
 template <int NPAD, int NT>
@@ -144,6 +181,20 @@ inline DaySplit split_days(int nd, int64_t cblocks, int ctas_per_sm, int min_per
   if (pairs) per = (per + 1) & ~1;
   if (per > nd) per = nd;
   return {(nd + per - 1) / per, per};
+}
+
+// Time split of the streaming quantile-mapping kernels: blockIdx.y walks `chunks` chunks of `rows` steps.  Enough
+// chunks for 16 CTAs per SM over the cblocks cell blocks, each at least min_rows steps, rounded up to whole `align`s.
+struct RowSplit {
+  int chunks, rows;
+};
+inline RowSplit split_rows(int64_t T, int64_t cblocks, int align, int min_rows) {
+  int64_t chunks = (sm_count() * 16 + cblocks - 1) / cblocks;
+  if (chunks < 1) chunks = 1;
+  int64_t rows = (T + chunks - 1) / chunks;
+  rows = (rows + align - 1) / align * align;
+  if (rows < min_rows) rows = min_rows;
+  return {(int)((T + rows - 1) / rows), (int)rows};
 }
 
 }  // namespace xc

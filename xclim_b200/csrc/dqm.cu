@@ -21,15 +21,15 @@
 // coefficients.  The sums run in time order within a lane, so the coefficients are deterministic.
 //
 // The file is compiled with -fmad=false (_build.EXTRA_FLAGS): the trend, the detrend and the retrend are then the
-// float64 operations of the oracle one by one, bit for bit given the same coefficients.  The interpolation repeats
-// qdm_apply_kernel's two-weight form and nearest bounds and eqm_adjust_kernel's position table instead of sharing
-// them: those kernels are compiled with fused multiply-adds allowed, and moving their device code into a header
-// would tie their code generation to this file's.
+// float64 operations of the oracle one by one, bit for bit given the same coefficients.  The interpolation, the
+// position table and the row loop come from qmap.cuh, shared with the kernels compiled with fused multiply-adds
+// allowed: that code is explicit rounding intrinsics, comparisons and integer arithmetic only, so -fmad cannot
+// change it.
 #include <float.h>
 
 #include <algorithm>
 
-#include "common.cuh"
+#include "qmap.cuh"
 
 namespace xc {
 namespace {
@@ -189,20 +189,10 @@ poly_fit_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t ldx, 
   }
 }
 
-// rows of a (cell block, time chunk) grid: enough CTAs for ~16 per SM, at least 64 rows per CTA
-inline int split_rows(int64_t T, int64_t cblocks, int* tchunks) {
-  int tc = (int)((sm_count() * 16 + cblocks - 1) / cblocks);
-  tc = tc < 1 ? 1 : tc;
-  int64_t rows = (T + tc - 1) / tc;
-  if (rows < 64) rows = 64;
-  *tchunks = (int)((T + rows - 1) / rows);
-  return (int)rows;
-}
-
 // adjust: a lane owns a cell and streams rows [t0, t1) of it.  Per lane, in shared memory (column = lane): the search
 // keys (linear: the compacted hist_q; nearest: interp1d's bounds between them), the compacted af, and a 32-entry
 // position table lut[b] = #{keys in a lower bin than b}, a lower bound of #{keys < d} for d in bin b (the bins are a
-// monotone function of the value), from which a short forward scan finds the segment.
+// monotone function of the value, qmap::PosTable), from which a short forward scan finds the segment.
 template <int INTERP, int KIND>
 __global__ void __launch_bounds__(kAdjThreads)
 dqm_adjust_kernel(const float* __restrict__ sim, int64_t T, int64_t C, int64_t ldx, const float* __restrict__ af,
@@ -223,8 +213,7 @@ dqm_adjust_kernel(const float* __restrict__ sim, int64_t T, int64_t C, int64_t l
     if (h == h && a == a) {
       if (m == 0) x_first = h;
       if (INTERP == 1) ks[m * kAdjThreads + lane] = h;
-      // interp1d(kind="nearest"): x_bds = x / 2; x_bds[1:] + x_bds[:-1], in float32
-      else if (m > 0) ks[(m - 1) * kAdjThreads + lane] = __fadd_rn(__fmul_rn(h, 0.5f), __fmul_rn(xprev, 0.5f));
+      else if (m > 0) ks[(m - 1) * kAdjThreads + lane] = qmap::nearest_bound(xprev, h);   // interp1d's nearest bounds
       ys[m * kAdjThreads + lane] = a;
       xprev = h;
       x_last = h;
@@ -234,41 +223,19 @@ dqm_adjust_kernel(const float* __restrict__ sim, int64_t T, int64_t C, int64_t l
   const int nk = (INTERP == 1) ? m : m - 1;   // search keys
   const double k_first = nk > 0 ? (double)ks[lane] : 0.0;
   const double k_range = nk > 0 ? (double)ks[(nk - 1) * kAdjThreads + lane] - k_first : 0.0;
-  const double scale = (nk >= 2 && k_range > 0.0 && k_range < INFINITY) ? (double)kLut / k_range : 0.0;
-  auto bin_of = [&](double v) -> int {
-    const double b = (v - k_first) * scale;
-    return b >= (double)(kLut - 1) ? kLut - 1 : (b > 0.0 ? (int)b : 0);
-  };
-  for (int b = 0; b < kLut; ++b) lut[b * kAdjThreads + lane] = 0;
-  for (int j = 0; j < nk; ++j) {      // histogram of the keys' bins, then exclusive prefix
-    const int b = bin_of((double)ks[j * kAdjThreads + lane]);
-    lut[b * kAdjThreads + lane] += 1;
-  }
-  int run = 0;
-  for (int b = 0; b < kLut; ++b) {
-    const int k = lut[b * kAdjThreads + lane];
-    lut[b * kAdjThreads + lane] = (unsigned char)run;
-    run += k;
-  }
+  const qmap::PosTable<double, kAdjThreads, kLut, false> pos(ks + lane, lut + lane, k_first, k_range, nk >= 2);
+  pos.build(nk, true);
   auto factor = [&](double q) -> float {
-    if (!(q == q) || m == 0) return NAN;
-    if (INTERP == 1) {
-      if (q < (double)x_first) return ys[lane];                                     // fill_value below
-      if (q > (double)x_last) return ys[(m - 1) * kAdjThreads + lane];              // ... and above
-      if (m == 1) return NAN;   // one node: interp1d's slope 0 / 0 at the node itself
-    }
-    // i = #{keys < q} (searchsorted side="left")
-    int i = lut[bin_of(q) * kAdjThreads + lane];
-    while (i < nk && (double)ks[i * kAdjThreads + lane] < q) ++i;
+    float f;
+    if (qmap::interp1d_edges<INTERP>(q, m, [&] { return x_first; }, [&] { return x_last; },
+                                     [&](int i) { return ys[i * kAdjThreads + lane]; }, f))
+      return f;
+    int i = pos.count_below(q, nk);
     if (INTERP == 1) {
       i = min(max(i, 1), m - 1);
       const float x0 = ks[(i - 1) * kAdjThreads + lane], x1 = ks[i * kAdjThreads + lane];
       const float y0 = ys[(i - 1) * kAdjThreads + lane], y1 = ys[i * kAdjThreads + lane];
-      // interp1d's two-weight form ((x_new - x_lo) / dx) * y_hi + ((x_hi - x_new) / dx) * y_lo, dx = x_hi - x_lo
-      // in float32 (both nodes are float32), the rest in float64
-      const double dx = (double)__fsub_rn(x1, x0);
-      const double w1 = __ddiv_rn(__dsub_rn(q, (double)x0), dx), w0 = __ddiv_rn(__dsub_rn((double)x1, q), dx);
-      return __double2float_rn(__dadd_rn(__dmul_rn(w1, (double)y1), __dmul_rn(w0, (double)y0)));
+      return qmap::linear_two_weight(q, x0, x1, y0, y1);
     }
     return ys[i * kAdjThreads + lane];   // nearest: ties to the lower node
   };
@@ -285,25 +252,7 @@ dqm_adjust_kernel(const float* __restrict__ sim, int64_t T, int64_t C, int64_t l
     return (float)((KIND == 0) ? (d + f) + tau : (d * f) * tau);
   };
   const int64_t t0 = (int64_t)blockIdx.y * rows_per_block;
-  const int64_t t1 = min(T, t0 + rows_per_block);
-  constexpr int U = 8;
-  int64_t t = t0;
-  const float* ps = sim + t0 * ldx + c;
-  float* po = scen + t0 * C + c;
-  for (; t + U <= t1; t += U) {
-    float xv[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) xv[u] = ld_stream(ps + (int64_t)u * ldx);
-#pragma unroll
-    for (int u = 0; u < U; ++u) po[(int64_t)u * C] = one(xv[u], t + u);
-    ps += (int64_t)U * ldx;
-    po += (int64_t)U * C;
-  }
-  for (; t < t1; ++t) {
-    *po = one(ld_stream(ps), t);
-    ps += ldx;
-    po += C;
-  }
+  qmap::stream_rows<8>(sim + c, ldx, scen + c, C, t0, min(T, t0 + rows_per_block), one);
 }
 
 // generic.detrend: out = x - tau in float64, a lane per cell, rows [t0, t1)
@@ -316,25 +265,8 @@ detrend_apply_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t 
   const double c1 = deg >= 1 ? coef[C + c] : 0.0;
   const double c2 = deg >= 2 ? coef[2 * C + c] : 0.0;
   const int64_t t0 = (int64_t)blockIdx.y * rows_per_block;
-  const int64_t t1 = min(T, t0 + rows_per_block);
-  constexpr int U = 8;
-  int64_t t = t0;
-  const float* ps = x + t0 * ldx + c;
-  double* po = out + t0 * C + c;
-  for (; t + U <= t1; t += U) {
-    float xv[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) xv[u] = ld_stream(ps + (int64_t)u * ldx);
-#pragma unroll
-    for (int u = 0; u < U; ++u) po[(int64_t)u * C] = (double)xv[u] - trend_at(c0, c1, c2, deg, basis_u(t + u, T));
-    ps += (int64_t)U * ldx;
-    po += (int64_t)U * C;
-  }
-  for (; t < t1; ++t) {
-    *po = (double)ld_stream(ps) - trend_at(c0, c1, c2, deg, basis_u(t, T));
-    ps += ldx;
-    po += C;
-  }
+  qmap::stream_rows<8>(x + c, ldx, out + c, C, t0, min(T, t0 + rows_per_block),
+                       [&](float v, int64_t t) { return (double)v - trend_at(c0, c1, c2, deg, basis_u(t, T)); });
 }
 
 }  // namespace
@@ -378,27 +310,14 @@ extern "C" int32_t xc_dqm_adjust_f32(const float* sim, int64_t T, int64_t C, int
                                      int32_t kind, int32_t interp, int32_t degree, float* scen, void* stream) {
   XC_REQUIRE(sim && af && hist_q && scaling && coef && scen, "null pointer argument");
   if (int32_t e = check_series(sim, T, C, ldx, degree)) return e;
-  XC_REQUIRE(nq >= 2 && nq <= 200, "nquantiles must be in [2, 200]");   // node counts fit the 8-bit position table
-  XC_REQUIRE(kind == 0 || kind == 1, "kind must be 0 ('+') or 1 ('*')");
-  XC_REQUIRE(interp == 0 || interp == 1, "interp must be 0 (nearest) or 1 (linear)");
-  cudaStream_t st = (cudaStream_t)stream;
+  if (int32_t e = check_qmap_args(nq, 2, 200, kind, interp)) return e;   // node counts fit the 8-bit position table
   const int64_t cblocks = (C + kAdjThreads - 1) / kAdjThreads;
-  int tchunks = 1;
-  const int rows = split_rows(T, cblocks, &tchunks);
+  const RowSplit split = split_rows(T, cblocks, 1, 64);
   const size_t smem = (size_t)2 * nq * kAdjThreads * 4 + (size_t)kLut * kAdjThreads;
-  const dim3 grid((unsigned)cblocks, (unsigned)tchunks, 1);
-#define XC_DQM_ADJ(I, K)                                                                                           \
-  do {                                                                                                             \
-    XC_CHECK_CUDA(cudaFuncSetAttribute(dqm_adjust_kernel<I, K>, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
-                                       (int)smem));                                                                \
-    dqm_adjust_kernel<I, K><<<grid, kAdjThreads, smem, st>>>(sim, T, C, ldx, af, hist_q, scaling, coef, nq, degree, \
-                                                             rows, scen);                                          \
-  } while (0)
-  if (interp == 0 && kind == 0) XC_DQM_ADJ(0, 0);
-  else if (interp == 0) XC_DQM_ADJ(0, 1);
-  else if (kind == 0) XC_DQM_ADJ(1, 0);
-  else XC_DQM_ADJ(1, 1);
-#undef XC_DQM_ADJ
+  auto kernel = dispatch_interp_kind(interp, kind, [](auto I, auto K) { return dqm_adjust_kernel<I.value, K.value>; });
+  if (int32_t e = allow_smem(kernel, smem, "cudaFuncSetAttribute(dqm_adjust_kernel)")) return e;
+  kernel<<<dim3((unsigned)cblocks, (unsigned)split.chunks, 1), kAdjThreads, smem, (cudaStream_t)stream>>>(
+      sim, T, C, ldx, af, hist_q, scaling, coef, nq, degree, split.rows, scen);
   return launch_status("dqm_adjust_kernel");
 }
 
@@ -406,11 +325,9 @@ extern "C" int32_t xc_detrend_apply_f32(const float* x, int64_t T, int64_t C, in
                                         int32_t degree, double* out, void* stream) {
   XC_REQUIRE(x && coef && out, "null pointer argument");
   if (int32_t e = check_series(x, T, C, ldx, degree)) return e;
-  cudaStream_t st = (cudaStream_t)stream;
   const int64_t cblocks = (C + kAdjThreads - 1) / kAdjThreads;
-  int tchunks = 1;
-  const int rows = split_rows(T, cblocks, &tchunks);
-  detrend_apply_kernel<<<dim3((unsigned)cblocks, (unsigned)tchunks, 1), kAdjThreads, 0, st>>>(x, T, C, ldx, coef,
-                                                                                            degree, rows, out);
+  const RowSplit split = split_rows(T, cblocks, 1, 64);
+  detrend_apply_kernel<<<dim3((unsigned)cblocks, (unsigned)split.chunks, 1), kAdjThreads, 0, (cudaStream_t)stream>>>(
+      x, T, C, ldx, coef, degree, split.rows, out);
   return launch_status("detrend_apply_kernel");
 }

@@ -8,17 +8,16 @@
 //   adjust: scen = sim (+|*) interp(sim; hist_q -> af), nearest or linear, constant extrapolation.
 // Reference call sites: tests/test_xsdba.py:21-34, 143-150.
 //
-// Design.  train needs ~2*nq order statistics spread over the WHOLE distribution of a
-// 10950-sample series, i.e. a real per-cell sort: one CTA owns one cell, gathers its series into
-// shared memory (64 KB for 16384 keys) and runs a bitonic sort there; neighbouring cells are
-// handled by neighbouring CTAs at the same time so that the 32-byte sectors fetched by the strided
-// gather are shared through L2.  adjust is a streaming pass: a lane owns one cell, keeps the 2*nq
-// table entries of its cell in a conflict-free shared-memory column and does a binary search per
-// element.
+// Design.  train needs ~2*nq order statistics spread over the whole distribution of each series.  A CTA owns a
+// group of 32 (or 16) adjacent cells and selects them without sorting: min / max, a 1024-bin histogram, the bins
+// of the wanted ranks, then a rank by counting inside those bins (eqm_train_group_kernel).  The cells it cannot
+// finish go to a one-cell-per-CTA kernel with the same selection and a bitonic-sort fallback (eqm_train_kernel).
+// adjust is a streaming pass: a lane owns one cell, keeps its quantile table in a conflict-free shared-memory
+// column and finds the segment of each element through a 32-entry position table (qmap.cuh).
 #include <float.h>
 #include <stdlib.h>
 
-#include "common.cuh"
+#include "qmap.cuh"
 
 namespace xc {
 namespace {
@@ -124,16 +123,8 @@ eqm_train_kernel(const float* __restrict__ ref, const float* __restrict__ hist, 
       __syncthreads();
       // ---- wanted order statistics: ranks ilo, ihi of every quantile
       for (int g = tid; g < ntg; g += kSortThreads) {
-        const int j = g >> 1;
-        // nodes are cast to the data dtype before use (xsdba: equally_spaced_nodes(n).astype(ref.dtype))
-        const double q = (double)(float)(((double)j + 0.5) / (double)nq);
-        const int ilo = (int)floor(q * (double)(n - 1));
-        const int r = (g & 1) ? min(ilo + 1, n - 1) : ilo;
-        int lo = 0, hi = kBins;  // bin b with prefix[b] <= r < prefix[b+1]
-        while (hi - lo > 1) {
-          const int mid = (lo + hi) >> 1;
-          if (hist_s[mid] <= r) lo = mid; else hi = mid;
-        }
+        const int r = qmap::target_rank(g, nq, n);
+        const int lo = qmap::bin_of_rank(r, kBins, [&](int b) { return hist_s[b]; });
         tgt_bin[g] = lo;
         tgt_rank[g] = r - hist_s[lo];
         if (atomicCAS(&slot_of_bin[lo], -1, -2) == -1) {  // first to claim the bin allocates its slot
@@ -189,21 +180,7 @@ eqm_train_kernel(const float* __restrict__ ref, const float* __restrict__ hist, 
           continue;
         }
         if (m > kCap) continue;  // resolved by the sort below
-        const int want = tgt_rank[g];
-        float found = NAN;
-        for (int i = lane; i < m; i += 32) {
-          const float vi = cl[i];
-          int less = 0;
-          for (int k = 0; k < m; ++k) {
-            const float vk = cl[k];
-            less += (vk < vi || (vk == vi && k < i)) ? 1 : 0;
-          }
-          if (less == want) found = vi;
-        }
-        for (int o = 16; o > 0; o >>= 1) {
-          const float other = __shfl_xor_sync(0xffffffffu, found, o);
-          found = (found == found) ? found : other;
-        }
+        const float found = qmap::select_in_bin<false>(cl, m, tgt_rank[g], -1, lane).x;
         if (lane == 0) tgt_val[g] = found;
       }
       __syncthreads();
@@ -225,24 +202,10 @@ eqm_train_kernel(const float* __restrict__ ref, const float* __restrict__ hist, 
     for (int j = tid; j < nq; j += kSortThreads) {
       float qv = NAN;
       if (n > 0) {
-        if (degenerate) {
-          qv = mn;  // every valid value equals mn (or the range is not finite: not supported, gives mn)
-        } else {
-          const double q = (double)(float)(((double)j + 0.5) / (double)nq);
-          const double pos = q * (double)(n - 1);
-          const double lo = floor(pos);
-          const double g = pos - lo;
-          const double a0 = (double)tgt_val[2 * j], a1 = (double)tgt_val[2 * j + 1];
-          const double d = a1 - a0;
-          qv = (float)((g >= 0.5) ? (a1 - d * (1.0 - g)) : (a0 + d * g));
-        }
+        if (degenerate) qv = mn;  // every valid value equals mn (or the range is not finite: not supported, gives mn)
+        else qv = qmap::lerp_quantile(j, nq, n, tgt_val[2 * j], tgt_val[2 * j + 1]);
       }
-      if (pass == 0) {
-        refq[j] = qv;
-      } else {
-        hist_q[(int64_t)j * C + c] = qv;
-        af[(int64_t)j * C + c] = (kind == 0) ? (refq[j] - qv) : (refq[j] / qv);
-      }
+      qmap::store_quantile(pass, kind, qv, refq[j], hist_q, af, (int64_t)j * C + c);
     }
     __syncthreads();
   }
@@ -273,8 +236,8 @@ eqm_train_kernel(const float* __restrict__ ref, const float* __restrict__ hist, 
 // a candidate total beyond the pool, or a range so small that the scale overflows -- is appended to a redo
 // list that the one-cell kernel resolves with its full machinery (sort fallback included): the results are
 // those of eqm_train_kernel bit for bit.
-// Instantiations: <32, 1024> default; <32, 512>; <16, 512> when C is a multiple of 16 only or the targets of
-// 32 cells do not fit (nq > 40).
+// Instantiations: <32, 1024> by default; <16, 512> when C is a multiple of 16 only or the targets of 32 cells do
+// not fit (nq > 40).
 // NORM (DQM): the ranks are selected on the raw series and the two order statistics of a quantile (or the
 // constant of a degenerate cell) are normalised before the lerp, which equals selecting them on the normalised
 // series when the transform is monotone (norm_monotone).  Cells where it is not, and cells where the raw or the
@@ -469,15 +432,8 @@ eqm_train_group_kernel(const float* __restrict__ ref, const float* __restrict__ 
       const int cc = g / ntg, k = g - cc * ntg;
       const int nn = cell_n[cc];
       if (nn <= 0 || cell_scale[cc] == 0.f || c0 + cc >= C) continue;
-      const int j = k >> 1;
-      const double q = (double)(float)(((double)j + 0.5) / (double)nq);
-      const int ilo = (int)floor(q * (double)(nn - 1));
-      const int r = (k & 1) ? min(ilo + 1, nn - 1) : ilo;
-      int lo = 0, hi = kBins;  // bin b with prefix[b] <= r < prefix[b+1]
-      while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (pref_at(cc, mid) <= r) lo = mid; else hi = mid;
-      }
+      const int r = qmap::target_rank(k, nq, nn);
+      const int lo = qmap::bin_of_rank(r, kBins, [&](int b) { return pref_at(cc, b); });
       const int below = pref_at(cc, lo);
       tgt_bin[cc * ntg + k] = lo;
       tgt_rank[cc * ntg + k] = r - below;
@@ -562,28 +518,10 @@ eqm_train_group_kernel(const float* __restrict__ ref, const float* __restrict__ 
         }
         const int m = slot_n[cc * ntg + sl];
         const float* cl = reinterpret_cast<const float*>(un) + cc * kPool + off;
-        const int want0 = tgt_rank[k0 + h];
-        const int want1 = both ? tgt_rank[k0 + 1] : -1;
-        float f0 = NAN, f1 = NAN;
-        for (int i = lane; i < m; i += 32) {
-          const float vi = cl[i];
-          int less = 0;
-          for (int kk = 0; kk < m; ++kk) {
-            const float vk = cl[kk];
-            less += (vk < vi || (vk == vi && kk < i)) ? 1 : 0;
-          }
-          if (less == want0) f0 = vi;
-          if (less == want1) f1 = vi;
-        }
-        for (int o = 16; o > 0; o >>= 1) {
-          const float o0 = __shfl_xor_sync(0xffffffffu, f0, o);
-          const float o1 = __shfl_xor_sync(0xffffffffu, f1, o);
-          f0 = (f0 == f0) ? f0 : o0;
-          f1 = (f1 == f1) ? f1 : o1;
-        }
+        const float2 f = qmap::select_in_bin<true>(cl, m, tgt_rank[k0 + h], both ? tgt_rank[k0 + 1] : -1, lane);
         if (lane == 0) {
-          tgt_val[k0 + h] = f0;
-          if (both) tgt_val[k0 + 1] = f1;
+          tgt_val[k0 + h] = f.x;
+          if (both) tgt_val[k0 + 1] = f.y;
         }
       }
     }
@@ -599,27 +537,16 @@ eqm_train_group_kernel(const float* __restrict__ ref, const float* __restrict__ 
           qv = cell_mn[cc];  // every valid value equals mn (or the range is not finite: not supported, gives mn)
           if constexpr (NORM) qv = norm_apply(qv, kind, norm[(int64_t)pass * C + c0 + cc]);
         } else if (!bad_cell[cc]) {
-          const double q = (double)(float)(((double)j + 0.5) / (double)nq);
-          const double pos = q * (double)(nn - 1);
-          const double lo = floor(pos);
-          const double gq = pos - lo;
           float v0 = tgt_val[cc * ntg + 2 * j], v1 = tgt_val[cc * ntg + 2 * j + 1];
           if constexpr (NORM) {
             const float nc = norm[(int64_t)pass * C + c0 + cc];
             v0 = norm_apply(v0, kind, nc);
             v1 = norm_apply(v1, kind, nc);
           }
-          const double a0 = (double)v0, a1 = (double)v1;
-          const double d = a1 - a0;
-          qv = (float)((gq >= 0.5) ? (a1 - d * (1.0 - gq)) : (a0 + d * gq));
+          qv = qmap::lerp_quantile(j, nq, nn, v0, v1);
         }
       }
-      if (pass == 0) {
-        refq[cc][j] = qv;
-      } else {
-        hist_q[(int64_t)j * C + c0 + cc] = qv;
-        af[(int64_t)j * C + c0 + cc] = (kind == 0) ? (refq[cc][j] - qv) : (refq[cc][j] / qv);
-      }
+      qmap::store_quantile(pass, kind, qv, refq[cc][j], hist_q, af, (int64_t)j * C + c0 + cc);
     }
     __syncthreads();
     // a cell that could not be finished goes to the redo list (both passes are redone there)
@@ -636,11 +563,9 @@ constexpr int kAdjThreads = 128;
 constexpr int kLut = 32;   // coarse position table per cell
 
 // adjust: a lane owns a cell and streams its series.  Per element the segment of the quantile table is found
-// through a 32-entry position table of the cell instead of a 5-step bisection (~45 instructions per element,
-// issue-bound): b = bin(x) on a uniform grid over [hq[0], hq[nq-1]],
-// lut[b] = #{ j : bin(hq[j]) < b } is a LOWER bound of idx = #{ hq[j] < x } (bin() is monotone, so a node in a
-// lower bin is below x), and the few nodes sharing x's bin are settled by a short forward scan -- two
-// unconditional steps, then a loop that almost never runs.  Same idx, same arithmetic, bit-identical output.
+// through a 32-entry position table of the cell (qmap::PosTable over [hq[0], hq[nq-1]]) instead of a 5-step
+// bisection (~45 instructions per element, issue-bound): a lower bound from the table, then a short forward scan --
+// two unconditional steps, then a loop that almost never runs.
 template <int INTERP, int KIND>
 __global__ void __launch_bounds__(kAdjThreads)
 eqm_adjust_kernel(const float* __restrict__ sim, int64_t T, int64_t C, int64_t ldx, const float* __restrict__ af,
@@ -670,33 +595,13 @@ eqm_adjust_kernel(const float* __restrict__ sim, int64_t T, int64_t C, int64_t l
   const int64_t t1 = min(T, t0 + rows_per_block);
   const float h_first = hq[lane], h_last = hq[(nq - 1) * kAdjThreads + lane];
   const float a_first = fa[lane], a_last = fa[(nq - 1) * kAdjThreads + lane];
-  // position table (degenerate or non-finite ranges: scale 0 -> every x in bin 0 -> plain forward scan)
-  const float range = h_last - h_first;
-  const float scale = (!bad && range > 0.f && range < INFINITY) ? (float)kLut / range : 0.f;
-  auto bin_of = [&](float x) -> int { return max(0, min(kLut - 1, (int)((x - h_first) * scale))); };
-  for (int b = 0; b < kLut; ++b) lut[b * kAdjThreads + lane] = 0;
-  if (!bad) {
-    for (int j = 0; j < nq; ++j) {      // histogram of the nodes' bins, then exclusive prefix
-      const int b = bin_of(hq[j * kAdjThreads + lane]);
-      lut[b * kAdjThreads + lane] += 1;
-    }
-    int run = 0;
-    for (int b = 0; b < kLut; ++b) {
-      const int n = lut[b * kAdjThreads + lane];
-      lut[b * kAdjThreads + lane] = (unsigned char)run;
-      run += n;
-    }
-  }
+  const qmap::PosTable<float, kAdjThreads, kLut, true> pos(hq + lane, lut + lane, h_first, h_last - h_first, !bad);
+  pos.build(nq, !bad);
   auto factor = [&](float x) -> float {
     if (bad || x != x) return NAN;
     if (x <= h_first) return a_first;
     if (x >= h_last) return a_last;
-    // idx = #{hq < x} (searchsorted side="left"): lower bound from the table, forward scan inside the bin
-    int idx = lut[bin_of(x) * kAdjThreads + lane];
-#pragma unroll
-    for (int k = 0; k < 2; ++k) idx += (idx < nq && hq[min(idx, nq - 1) * kAdjThreads + lane] < x) ? 1 : 0;
-    while (idx < nq && hq[idx * kAdjThreads + lane] < x) ++idx;
-    idx = max(1, min(idx, nq - 1));
+    const int idx = max(1, min(pos.count_below(x, nq), nq - 1));
     const float x0 = hq[(idx - 1) * kAdjThreads + lane];
     const float y0 = fa[(idx - 1) * kAdjThreads + lane];
     if (INTERP == 1) {
@@ -708,6 +613,7 @@ eqm_adjust_kernel(const float* __restrict__ sim, int64_t T, int64_t C, int64_t l
     const float mid = __fmul_rn(__fadd_rn(x0, x1), 0.5f);
     return (x <= mid) ? y0 : y1;
   };
+  // all U factors of a batch before its stores (qmap::stream_rows interleaves them, which compiles worse here)
   constexpr int U = 16;  // rows in flight per lane: shared memory caps the CTAs per SM at 6, so the bytes in flight come from here
   int64_t t = t0;
   const float* ps = sim + t0 * ldx + c;
@@ -765,41 +671,21 @@ extern "C" int64_t xc_eqm_train_workspace_bytes(int64_t T, int64_t C, int32_t nq
 static int32_t launch_train_cells(const float* ref, const float* hist, int64_t T, int64_t C, int64_t ldx, int32_t nq,
                                   int32_t kind, float* af, float* hist_q, const int32_t* redo, unsigned grid,
                                   const float* norm, cudaStream_t st) {
-  int npad = 1024;
-  while (npad < T) npad <<= 1;
-  const size_t smem = ((size_t)npad + ((nq + 3) & ~3) + (size_t)2 * nq * kCap) * 4;
-  auto go = [&](auto NORMC) -> int32_t {
-    constexpr bool NORM = decltype(NORMC)::value;
-#define XC_TRAIN(NP)                                                                                               \
-  do {                                                                                                             \
-    if (smem > 48 * 1024) {                                                                                        \
-      cudaError_t e_ = cudaFuncSetAttribute(eqm_train_kernel<NP, NORM>, cudaFuncAttributeMaxDynamicSharedMemorySize,\
-                                            (int)smem);                                                            \
-      if (e_ != cudaSuccess) return cuda_fail(e_, "cudaFuncSetAttribute(eqm_train_kernel)");                       \
-    }                                                                                                              \
-    eqm_train_kernel<NP, NORM><<<grid, kSortThreads, smem, st>>>(ref, hist, (int32_t)T, C, ldx, nq, kind, af,      \
-                                                                 hist_q, redo, norm);                              \
-  } while (0)
-    switch (npad) {
-      case 1024: XC_TRAIN(1024); break;
-      case 2048: XC_TRAIN(2048); break;
-      case 4096: XC_TRAIN(4096); break;
-      case 8192: XC_TRAIN(8192); break;
-      case 16384: XC_TRAIN(16384); break;
-      default: XC_TRAIN(32768); break;
-    }
-#undef XC_TRAIN
+  return dispatch_npad(T, [&](auto NP) -> int32_t {
+    constexpr int NPAD = decltype(NP)::value;
+    const size_t smem = ((size_t)NPAD + ((nq + 3) & ~3) + (size_t)2 * nq * kCap) * 4;
+    auto kernel = norm ? eqm_train_kernel<NPAD, true> : eqm_train_kernel<NPAD, false>;
+    if (int32_t e = allow_smem(kernel, smem, "cudaFuncSetAttribute(eqm_train_kernel)")) return e;
+    kernel<<<grid, kSortThreads, smem, st>>>(ref, hist, (int32_t)T, C, ldx, nq, kind, af, hist_q, redo, norm);
     return launch_status("eqm_train_kernel");
-  };
-  return norm ? go(std::true_type{}) : go(std::false_type{});
+  });
 }
 
 static int32_t check_train_args(const float* ref, const float* hist, int64_t T, int64_t C, int64_t ldx, int32_t nq,
                                 int32_t kind, const float* af, const float* hist_q, const char* who) {
   XC_REQUIRE(ref && hist && af && hist_q, "null pointer argument");
   XC_REQUIRE(T > 0 && C > 0 && ldx >= C, "bad shape");
-  XC_REQUIRE(nq >= 1 && nq <= 64, "nquantiles must be in [1, 64]");
-  XC_REQUIRE(kind == 0 || kind == 1, "kind must be 0 ('+') or 1 ('*')");
+  if (int32_t e = check_qmap_args(nq, 1, 64, kind)) return e;
   XC_REQUIRE(C <= 2147483647LL, "too many cells for one launch");
   if (T > 32768) {
     set_error("%s: series longer than 32768 steps do not fit the shared-memory sort", who);
@@ -816,11 +702,7 @@ static int32_t train_impl(const float* ref, const float* hist, int64_t T, int64_
   // widest group first: 32 cells = 128 bytes per (CTA, time row) touch; 16 when C is not a multiple of 32 or the
   // targets of 32 cells do not fit in shared memory.  (A variant that staged a 4-cell slice in shared memory and
   // read DRAM once was slower -- four times the row touches -- and is gone.)
-  const char* kg_env = getenv("XCLIM_B200_EQM_KG");
-  const char* gt_env = getenv("XCLIM_B200_EQM_GT");
-  int g = 32;
-  if (kg_env && atoi(kg_env) == 16) g = 16;
-  if (g == 32 && (C % 32 != 0 || train_group_smem_bytes(32, 2 * nq) + 12 * 1024 > 227 * 1024)) g = 16;
+  const int g = (C % 32 != 0 || train_group_smem_bytes(32, 2 * nq) + 12 * 1024 > 227 * 1024) ? 16 : 32;
   const bool fits = train_group_smem_bytes(g, 2 * nq) + 8 * 1024 <= 227 * 1024;
   const bool vec_ok = (C % g == 0) && (ldx % 4 == 0) && aligned16(ref) && aligned16(hist);
   if (workspace == nullptr || workspace_bytes < need || !vec_ok || !fits || getenv("XCLIM_B200_EQM_V1")) {
@@ -832,23 +714,12 @@ static int32_t train_impl(const float* ref, const float* hist, int64_t T, int64_
   XC_CHECK_CUDA(cudaMemsetAsync(redo, 0, 4, st));
   const size_t smemg = train_group_smem_bytes(g, 2 * nq);
   const int64_t groups = C / g;
-  auto go = [&](auto NORMC) -> int32_t {
-    constexpr bool NORM = decltype(NORMC)::value;
-#define XC_TRAIN_GROUP(G, GT)                                                                                      \
-  do {                                                                                                             \
-    XC_CHECK_CUDA(cudaFuncSetAttribute(eqm_train_group_kernel<G, GT, NORM>,                                        \
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemg));                  \
-    eqm_train_group_kernel<G, GT, NORM><<<(unsigned)groups, GT, smemg, st>>>(ref, hist, (int32_t)T, C, ldx, nq,    \
-                                                                              kind, af, hist_q, redo, norm);       \
-  } while (0)
-    if (g == 32 && gt_env && atoi(gt_env) == 512) XC_TRAIN_GROUP(32, 512);
-    else if (g == 32) XC_TRAIN_GROUP(32, 1024);
-    else XC_TRAIN_GROUP(16, 512);
-#undef XC_TRAIN_GROUP
-    return launch_status("eqm_train_group_kernel");
-  };
-  int32_t e = norm ? go(std::true_type{}) : go(std::false_type{});
-  if (e) return e;
+  auto kernel = g == 32 ? (norm ? eqm_train_group_kernel<32, 1024, true> : eqm_train_group_kernel<32, 1024, false>)
+                        : (norm ? eqm_train_group_kernel<16, 512, true> : eqm_train_group_kernel<16, 512, false>);
+  if (int32_t e = allow_smem(kernel, smemg, "cudaFuncSetAttribute(eqm_train_group_kernel)")) return e;
+  kernel<<<(unsigned)groups, g == 32 ? 1024 : 512, smemg, st>>>(ref, hist, (int32_t)T, C, ldx, nq, kind, af, hist_q,
+                                                                 redo, norm);
+  if (int32_t e = launch_status("eqm_train_group_kernel")) return e;
   // cells the eight-cell layout could not finish (heavy non-constant bins): a small fixed grid walks the list
   return launch_train_cells(ref, hist, T, C, ldx, nq, kind, af, hist_q, redo, 2u * (unsigned)sm_count(), norm, st);
 }
@@ -866,32 +737,14 @@ extern "C" int32_t xc_eqm_adjust_f32(const float* sim, int64_t T, int64_t C, int
                                      void* stream) {
   XC_REQUIRE(sim && af && hist_q && scen, "null pointer argument");
   XC_REQUIRE(T > 0 && C > 0 && ldx >= C, "bad shape");
-  XC_REQUIRE(nq >= 2 && nq <= 200, "nquantiles must be in [2, 200]");   // node counts fit the 8-bit position table
-  XC_REQUIRE(kind == 0 || kind == 1, "kind must be 0 ('+') or 1 ('*')");
-  XC_REQUIRE(interp == 0 || interp == 1, "interp must be 0 (nearest) or 1 (linear)");
-  cudaStream_t st = (cudaStream_t)stream;
+  if (int32_t e = check_qmap_args(nq, 2, 200, kind, interp)) return e;   // node counts fit the 8-bit position table
   const int64_t cblocks = (C + kAdjThreads - 1) / kAdjThreads;
-  int tchunks = (int)((sm_count() * 16 + cblocks - 1) / cblocks);
-  tchunks = tchunks < 1 ? 1 : tchunks;
-  int rows = (int)((T + tchunks - 1) / tchunks);
-  if (rows < 64) rows = 64;
-  tchunks = (int)((T + rows - 1) / rows);
+  const RowSplit split = split_rows(T, cblocks, 1, 64);
   const size_t smem = (size_t)3 * nq * kAdjThreads * 4 + (size_t)kLut * kAdjThreads;
-  dim3 grid((unsigned)cblocks, (unsigned)tchunks, 1);
-#define XC_ADJ(I, K)                                                                                               \
-  do {                                                                                                             \
-    if (smem > 48 * 1024) {                                                                                        \
-      cudaError_t e_ = cudaFuncSetAttribute(eqm_adjust_kernel<I, K>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
-                                            (int)smem);                                                            \
-      if (e_ != cudaSuccess) return cuda_fail(e_, "cudaFuncSetAttribute(eqm_adjust_kernel)");                      \
-    }                                                                                                              \
-    eqm_adjust_kernel<I, K><<<grid, kAdjThreads, smem, st>>>(sim, T, C, ldx, af, hist_q, nq, rows, scen);          \
-  } while (0)
-  if (interp == 0 && kind == 0) XC_ADJ(0, 0);
-  else if (interp == 0) XC_ADJ(0, 1);
-  else if (kind == 0) XC_ADJ(1, 0);
-  else XC_ADJ(1, 1);
-#undef XC_ADJ
+  auto kernel = dispatch_interp_kind(interp, kind, [](auto I, auto K) { return eqm_adjust_kernel<I.value, K.value>; });
+  if (int32_t e = allow_smem(kernel, smem, "cudaFuncSetAttribute(eqm_adjust_kernel)")) return e;
+  kernel<<<dim3((unsigned)cblocks, (unsigned)split.chunks, 1), kAdjThreads, smem, (cudaStream_t)stream>>>(
+      sim, T, C, ldx, af, hist_q, nq, split.rows, scen);
   return launch_status("eqm_adjust_kernel");
 }
 

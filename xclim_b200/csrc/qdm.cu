@@ -39,7 +39,7 @@
 
 #include <algorithm>
 
-#include "common.cuh"
+#include "qmap.cuh"
 
 namespace xc {
 namespace {
@@ -286,9 +286,7 @@ qdm_apply_kernel(const float* __restrict__ sim, int64_t T, int64_t ldx, int64_t 
         const float a = af[(int64_t)j * ldaf + c];
         if (a == a) { xs[m * kTile + tx] = nodes[j]; ys[m * kTile + tx] = a; ++m; }
       }
-      // interp1d(kind="nearest"): x_bds = x / 2; x_bds[1:] + x_bds[:-1], in float32
-      for (int i = 0; i + 1 < m; ++i)
-        bd[i * kTile + tx] = __fadd_rn(__fmul_rn(xs[(i + 1) * kTile + tx], 0.5f), __fmul_rn(xs[i * kTile + tx], 0.5f));
+      for (int i = 0; i + 1 < m; ++i) bd[i * kTile + tx] = qmap::nearest_bound(xs[i * kTile + tx], xs[(i + 1) * kTile + tx]);
       const int4 st = stats[c];
       const double nd = (double)st.x;
       s_n[tx] = nd;
@@ -301,11 +299,11 @@ qdm_apply_kernel(const float* __restrict__ sim, int64_t T, int64_t ldx, int64_t 
   const int m = s_m[tx];
   const double nd = live ? s_n[tx] : 1.0, mn = live ? s_mn[tx] : 0.0, mx = live ? s_mx[tx] : 1.0;
   auto factor = [&](double q) -> float {
-    if (!(q == q) || m == 0) return NAN;
+    float f;
+    if (qmap::interp1d_edges<INTERP>(q, m, [&] { return xs[tx]; }, [&] { return xs[(m - 1) * kTile + tx]; },
+                                     [&](int i) { return ys[i * kTile + tx]; }, f))
+      return f;
     if (INTERP == 1) {
-      if (q < (double)xs[tx]) return ys[tx];                                          // fill_value below
-      if (q > (double)xs[(m - 1) * kTile + tx]) return ys[(m - 1) * kTile + tx];      // ... and above
-      if (m == 1) return NAN;   // one node: interp1d's slope 0 / 0 at the node itself
       // i = #{xs < q} clipped to [1, m - 1] (searchsorted side="left"): a guess from the uniform nodes, then
       // exact steps (more than one only where af had NaN entries)
       int i = min(max((int)(q * nq + 0.5), 1), m - 1);
@@ -313,11 +311,7 @@ qdm_apply_kernel(const float* __restrict__ sim, int64_t T, int64_t ldx, int64_t 
       while (i < m - 1 && (double)xs[i * kTile + tx] < q) ++i;
       const float x0 = xs[(i - 1) * kTile + tx], x1 = xs[i * kTile + tx];
       const float y0 = ys[(i - 1) * kTile + tx], y1 = ys[i * kTile + tx];
-      // interp1d's two-weight form ((x_new - x_lo) / dx) * y_hi + ((x_hi - x_new) / dx) * y_lo, dx = x_hi - x_lo
-      // in float32 (both nodes are float32), the rest in float64
-      const double dx = (double)__fsub_rn(x1, x0);
-      const double w1 = __ddiv_rn(__dsub_rn(q, (double)x0), dx), w0 = __ddiv_rn(__dsub_rn((double)x1, q), dx);
-      return __double2float_rn(__dadd_rn(__dmul_rn(w1, (double)y1), __dmul_rn(w0, (double)y0)));
+      return qmap::linear_two_weight(q, x0, x1, y0, y1);
     }
     // nearest: i = #{bd < q} (ties to the lower node) in [0, m - 1]
     int i = min(max((int)(q * nq), 0), m - 1);
@@ -373,9 +367,7 @@ extern "C" int32_t xc_qdm_adjust_f32(const float* sim, int64_t T, int64_t C, int
                                      double* sim_q, void* workspace, int64_t workspace_bytes, void* stream) {
   XC_REQUIRE(sim && af && nodes && scen && workspace, "null pointer argument");
   XC_REQUIRE(T > 0 && C > 0 && ldx >= C, "bad shape");
-  XC_REQUIRE(nq >= 2 && nq <= 200, "nquantiles must be in [2, 200]");
-  XC_REQUIRE(kind == 0 || kind == 1, "kind must be 0 ('+') or 1 ('*')");
-  XC_REQUIRE(interp == 0 || interp == 1, "interp must be 0 (nearest) or 1 (linear)");
+  if (int32_t e = check_qmap_args(nq, 2, 200, kind, interp)) return e;
   XC_REQUIRE(C <= 2147483647LL, "too many cells for one launch");
   if (T > kMaxSteps) {
     set_error("qdm_adjust: series longer than 32768 steps do not fit the shared-memory ranking");
@@ -391,30 +383,16 @@ extern "C" int32_t xc_qdm_adjust_f32(const float* sim, int64_t T, int64_t C, int
   // (for whole tiles chunk_bytes(T, nc) is exactly nc * (6 T + 16))
   const int64_t all = (C + kTile - 1) / kTile * kTile;
   const int64_t cc = std::min(all, avail / (6 * T + 16) / kTile * kTile);
-  int npad = 1024;
-  while (npad < T) npad <<= 1;
-  const int K = npad / 4;
-  const size_t smem_rank = std::max((size_t)4 * npad, (size_t)4 * T + (size_t)4 * K + (size_t)K / 8);
+  size_t smem_rank = 0;
+  auto rank = dispatch_npad(T, [&](auto NP) {
+    constexpr int NPAD = decltype(NP)::value, K = NPAD / 4;
+    smem_rank = std::max((size_t)4 * NPAD, (size_t)4 * T + (size_t)4 * K + (size_t)K / 8);
+    return qdm_rank_kernel<NPAD>;
+  });
   const size_t smem_apply = (size_t)3 * nq * kTile * 4;
-#define XC_RANK_ATTR(NP)                                                                                           \
-  XC_CHECK_CUDA(cudaFuncSetAttribute(qdm_rank_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_rank))
-  switch (npad) {
-    case 1024: XC_RANK_ATTR(1024); break;
-    case 2048: XC_RANK_ATTR(2048); break;
-    case 4096: XC_RANK_ATTR(4096); break;
-    case 8192: XC_RANK_ATTR(8192); break;
-    case 16384: XC_RANK_ATTR(16384); break;
-    default: XC_RANK_ATTR(32768); break;
-  }
-#undef XC_RANK_ATTR
-#define XC_APPLY_ATTR(I, KD)                                                                                       \
-  XC_CHECK_CUDA(cudaFuncSetAttribute(qdm_apply_kernel<I, KD>, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
-                                     (int)smem_apply))
-  if (interp == 0 && kind == 0) XC_APPLY_ATTR(0, 0);
-  else if (interp == 0) XC_APPLY_ATTR(0, 1);
-  else if (kind == 0) XC_APPLY_ATTR(1, 0);
-  else XC_APPLY_ATTR(1, 1);
-#undef XC_APPLY_ATTR
+  auto apply = dispatch_interp_kind(interp, kind, [](auto I, auto KD) { return qdm_apply_kernel<I.value, KD.value>; });
+  if (int32_t e = allow_smem(rank, smem_rank, "cudaFuncSetAttribute(qdm_rank_kernel)")) return e;
+  if (int32_t e = allow_smem(apply, smem_apply, "cudaFuncSetAttribute(qdm_apply_kernel)")) return e;
   for (int64_t c0 = 0; c0 < C; c0 += cc) {
     const int64_t nc = std::min(cc, C - c0);
     float* xt = reinterpret_cast<float*>(base);
@@ -425,35 +403,13 @@ extern "C" int32_t xc_qdm_adjust_f32(const float* sim, int64_t T, int64_t C, int
         sim + c0, T, ldx, nc, xt);
     int32_t e = launch_status("qdm_transpose_kernel");
     if (e) return e;
-    switch (npad) {
-#define XC_RANK(NP) qdm_rank_kernel<NP><<<(unsigned)nc, kRankThreads, smem_rank, st>>>(xt, (int32_t)T, rk, stats)
-      case 1024: XC_RANK(1024); break;
-      case 2048: XC_RANK(2048); break;
-      case 4096: XC_RANK(4096); break;
-      case 8192: XC_RANK(8192); break;
-      case 16384: XC_RANK(16384); break;
-      default: XC_RANK(32768); break;
-#undef XC_RANK
-    }
+    rank<<<(unsigned)nc, kRankThreads, smem_rank, st>>>(xt, (int32_t)T, rk, stats);
     e = launch_status("qdm_rank_kernel");
     if (e) return e;
-    // time split: enough CTAs for 16 per SM when the chunk is narrow, at least 4 tiles of rows per CTA
-    int tchunks = (int)((sm_count() * 16 + tiles - 1) / tiles);
-    tchunks = tchunks < 1 ? 1 : tchunks;
-    int rows = (int)((T + tchunks - 1) / tchunks);
-    rows = (rows + kTile - 1) / kTile * kTile;
-    if (rows < 4 * kTile) rows = 4 * kTile;
-    tchunks = (int)((T + rows - 1) / rows);
-    const dim3 grid(tiles, (unsigned)tchunks), block(kTile, 8);
-    double* sq = sim_q ? sim_q + c0 : nullptr;
-#define XC_APPLY(I, KD)                                                                                            \
-  qdm_apply_kernel<I, KD><<<grid, block, smem_apply, st>>>(sim + c0, T, ldx, nc, C, af + c0, C, nodes, nq, rk,      \
-                                                          stats, rows, scen + c0, sq)
-    if (interp == 0 && kind == 0) XC_APPLY(0, 0);
-    else if (interp == 0) XC_APPLY(0, 1);
-    else if (kind == 0) XC_APPLY(1, 0);
-    else XC_APPLY(1, 1);
-#undef XC_APPLY
+    // time split: whole 32-row tiles, at least 4 of them per CTA
+    const RowSplit split = split_rows(T, tiles, kTile, 4 * kTile);
+    apply<<<dim3(tiles, (unsigned)split.chunks), dim3(kTile, 8), smem_apply, st>>>(
+        sim + c0, T, ldx, nc, C, af + c0, C, nodes, nq, rk, stats, split.rows, scen + c0, sim_q ? sim_q + c0 : nullptr);
     e = launch_status("qdm_apply_kernel");
     if (e) return e;
   }
