@@ -158,7 +158,7 @@ def main():
         tab = device.percentile_doy(tas, doy, yidx, YEAR, P, 5, [90.0], 1 / 3, 1 / 3)[0]
         poff_ms = np.concatenate([[0], np.cumsum(np.tile([31, 28, 31, 30, 31, 30, 31, 31, 30, 31, 30, 31], P))]).astype(np.int32)
         ms = timeit(lambda: device.doy_threshold_count(tas, poff_ms, doy, tab, _lib.OPS[">"]), a.steps)
-        report("doy_count_kernel (tx90p count, freq=MS: generic periods)", ms,
+        report("period_count_thr_kernel (tx90p count, freq=MS: generic periods)", ms,
                T * C * 4 + YEAR * C * 8 + (len(poff_ms) - 1) * C * 4)
         del tab
     if want("bootstrap"):

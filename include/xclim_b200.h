@@ -308,7 +308,7 @@ int32_t xc_doy_threshold_count_f32(const float* x, int64_t T, int64_t C, int64_t
 
 /* Same count for the common layout "n_years whole years of year_len steps starting at first_row,
  * day-of-year == position in the year" (noleap / 360_day with freq YS): out[y, c] for y < n_years.
- * Year-blocked so that each table row is read once per 6 years; needs C, ldx % 4 == 0 and 16-byte
+ * Year-blocked so that each table row is read once per 3 years; needs C, ldx % 4 == 0 and 16-byte
  * aligned buffers (use xc_doy_threshold_count_f32 otherwise). */
 int32_t xc_doy_threshold_count_years_f32(const float* x, int64_t T, int64_t C, int64_t ldx,
                                          int64_t first_row, int32_t n_years, int32_t year_len,

@@ -136,10 +136,13 @@ def test_tx90p_reference_known_answer_leap_year(cuda):
     assert out.values[0] == 30 and out.values[1] == 29 and out.values[5] == 25
 
 
-@pytest.mark.parametrize("op", [">", ">=", "<", "<="])
+@pytest.mark.parametrize("op", [">", ">=", "<", "<=", "==", "!="])
 def test_doy_count_year_blocked_kernel_exact_ties(cuda, op):
-    """The year-blocked kernel folds float64 thresholds to float32 by directed rounding: it must agree
-    with the float64 compare for thresholds equal to data values, one double-ulp off, +-0, inf, NaN."""
+    """Every float64-threshold count folds its thresholds to float32 by directed rounding (fold_f64): it must
+    agree with the float64 compare for thresholds equal to data values, one double-ulp off, +-0, inf, NaN --
+    through every threshold source (year-blocked table, day-of-year table with 4 and with 1 cell per thread,
+    per-cell and per-step arrays) and every way to the 1-cell layout (C % 4 != 0, ldx > C, a base pointer
+    one float off).  == and != have no year-blocked kernel: their yearly count takes the day-of-year kernel."""
     import torch
     from xclim_b200 import device, _lib
     rng = np.random.default_rng(15)
@@ -152,21 +155,48 @@ def test_doy_count_year_blocked_kernel_exact_ties(cuda, op):
     tab[5, :8] = [0.0, -0.0, np.inf, -np.inf, np.nan, 1e-300, -1e-300, 1e300]
     x[5, :8] = [0.0, -0.0, 1.0, -1.0, 0.0, 0.0, -0.0, 3e38]
     poff = np.arange(N + 1, dtype=np.int32) * L
-    doy = np.tile(np.arange(1, L + 1), N).astype(np.int16)
-    xd, td = torch.from_numpy(x).cuda(), torch.from_numpy(tab).cuda()
-    got, valid = device.doy_threshold_count(xd, poff, doy, td, _lib.OPS[op], want_valid=True)   # year-blocked
-    exp = O.threshold_count(x, op, tab[doy - 1], poff)
-    np.testing.assert_array_equal(got.cpu().numpy(), exp)
-    np.testing.assert_array_equal(valid.cpu().numpy(), np.stack([(~np.isnan(x[s:e])).sum(0) for s, e in zip(poff[:-1], poff[1:])]))
-    # generic kernel on the same data (odd number of cells forces the 2-cell float64-compare kernel)
-    got2, _ = device.doy_threshold_count(xd[:, :63].contiguous(), poff, doy, td[:, :63].contiguous(), _lib.OPS[op])
-    np.testing.assert_array_equal(got2.cpu().numpy(), exp[:, :63])
-    # monthly periods on 64 cells: the 4-cell generic kernel with folded thresholds
     month = np.concatenate([[0], np.cumsum(np.tile([31, 28, 31, 30, 31, 30, 31, 31, 30, 31, 30, 31], N))]).astype(np.int32)
-    got3, valid3 = device.doy_threshold_count(xd, month, doy, td, _lib.OPS[op], want_valid=True)
-    np.testing.assert_array_equal(got3.cpu().numpy(), O.threshold_count(x, op, tab[doy - 1], month))
-    np.testing.assert_array_equal(valid3.cpu().numpy(),
-                                  np.stack([(~np.isnan(x[s:e])).sum(0) for s, e in zip(month[:-1], month[1:])]))
+    doy = np.tile(np.arange(1, L + 1), N).astype(np.int16)
+    code = _lib.OPS[op]
+    xd, td = torch.from_numpy(x).cuda(), torch.from_numpy(tab).cuda()
+
+    def expect(thr, po, cols=slice(None)):
+        return O.threshold_count(x[:, cols], op, thr, po, constrain=[op])
+
+    def nvalid(po, cols=slice(None)):
+        return np.stack([(~np.isnan(x[s:e, cols])).sum(0) for s, e in zip(po[:-1], po[1:])])
+
+    def check(got, exp):
+        np.testing.assert_array_equal(got.cpu().numpy(), exp)
+
+    for po in (poff, month):                 # yearly: year-blocked (inequalities); monthly: 4 cells per thread
+        got, valid = device.doy_threshold_count(xd, po, doy, td, code, want_valid=True)
+        check(got, expect(tab[doy - 1], po))
+        check(valid, nvalid(po))
+    # the 1-cell layouts: an odd number of cells, a row stride of 65 floats, a base pointer 4 bytes past 16-byte alignment
+    wide = torch.full((L * N, 65), 9.0, dtype=torch.float32, device="cuda")
+    wide[:, :64] = xd
+    shifted = torch.full((L * N, 68), 9.0, dtype=torch.float32, device="cuda")
+    shifted[:, 1:65] = xd
+    layouts = [(xd[:, :63].contiguous(), slice(0, 63)), (wide[:, :64], slice(None)),
+               (shifted[:, 1:65], slice(None))]
+    assert layouts[1][0].stride(0) == 65 and layouts[2][0].data_ptr() % 16 == 4
+    for xv, cols in layouts:
+        tv = td[:, cols].contiguous()
+        for po in (poff, month):
+            got, valid = device.doy_threshold_count(xv, po, doy, tv, code, want_valid=True)
+            check(got, expect(tab[doy - 1][:, cols], po, cols))
+            check(valid, nvalid(po, cols))
+        # array thresholds: per step (T, C) and per cell (1, C), the latter from the rows holding the edge values
+        tstep = torch.from_numpy(tab[doy - 1][:, cols].copy()).cuda()
+        check(device.period_count_arr(xv, month, code, tstep, True), expect(tab[doy - 1][:, cols], month, cols))
+        for r in (5, 1, 2):
+            tcell = torch.from_numpy(tab[r:r + 1, cols].copy()).cuda()
+            check(device.period_count_arr(xv, month, code, tcell, False), expect(tab[r, cols], month, cols))
+    # the array thresholds with 4 cells per thread
+    check(device.period_count_arr(xd, poff, code, torch.from_numpy(tab[doy - 1].copy()).cuda(), True),
+          expect(tab[doy - 1], poff))
+    check(device.period_count_arr(xd, month, code, td[5:6].contiguous(), False), expect(tab[5], month))
 
 
 @pytest.mark.parametrize("calendar,years,window", [("noleap", 30, 5), ("standard", 20, 9), ("360_day", 40, 5)])

@@ -14,7 +14,6 @@ import numpy as np
 import torch
 
 from . import _lib, device
-from .calendar import adjust_table, table_on_device
 from .field import attrs_of
 from .generic import _unwrap, _wrap_periods
 from .options import OPTIONS, set_options
@@ -81,17 +80,13 @@ def tx90p(tasmax, tasmax_per, freq="YS", bootstrap=False, op=">", **indexer):
         attrs = attrs_of(out)
         attrs["units"] = "days"
         return _wrap_periods(tasmax, masked, cell_shape, other, ta, freq, attrs, dtype=np.float64, name="tx90p")
+    from .indices import _percentile_table_count
     code = _lib.op_code(op, (">", ">="))
-    x2d, cell_shape, other, ta = _unwrap(tasmax)
-    poff = ta.period_offsets(freq)
-    from .indices import _table_in_units_of
-    table = _table_in_units_of(table_on_device(tasmax_per, cell_shape, other, x2d.device), tasmax_per, tasmax)
-    table, doy_idx = adjust_table(table, ta)
-    cnt, valid = device.doy_threshold_count(x2d, poff, doy_idx, table, code, want_valid=True)
+    cnt, valid, (cell_shape, other, ta) = _percentile_table_count(tasmax, tasmax_per, code, freq, want_valid=True)
     attrs = attrs_of(tasmax)
     attrs.update(units="days", cell_methods="time: sum over days")
-    return _wrap_periods(tasmax, _mask_missing(cnt, valid, poff, ta.expected_period_lengths(freq)), cell_shape, other, ta, freq, attrs, dtype=np.float64,
-                         name="tx90p")
+    masked = _mask_missing(cnt, valid, ta.period_offsets(freq), ta.expected_period_lengths(freq))
+    return _wrap_periods(tasmax, masked, cell_shape, other, ta, freq, attrs, dtype=np.float64, name="tx90p")
 
 
 # ---- generic indicator wrapper ---------------------------------------------------------------------------

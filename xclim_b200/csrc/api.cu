@@ -22,22 +22,13 @@ int32_t cuda_fail(cudaError_t e, const char* what) {
 }
 
 float fold_threshold(int32_t op, double thr, int32_t cmp_f64) {
-  float f = (float)thr;  // round to nearest even, as numpy does for a weak Python scalar
-  if (!cmp_f64 || thr != thr || op > XC_OP_NE) return f;
-  const double fd = (double)f;
-  switch (op) {
-    case XC_OP_GT:  // x > thr  <=>  x > rd(thr)   (largest float32 <= thr)
-    case XC_OP_LE:  // x <= thr <=>  x <= rd(thr)
-      if (fd > thr) f = nextafterf(f, -INFINITY);
-      return f;
-    case XC_OP_GE:  // x >= thr <=>  x >= ru(thr)  (smallest float32 >= thr)
-    case XC_OP_LT:  // x < thr  <=>  x < ru(thr)
-      if (fd < thr) f = nextafterf(f, INFINITY);
-      return f;
-    case XC_OP_EQ:  // never equal to an unrepresentable threshold: NaN compares False
-    case XC_OP_NE:  // always different:                              NaN compares True
-      return fd == thr ? f : NAN;
-  }
+  // round to nearest even, as numpy does for a weak Python scalar (and for the NaN tests, which ignore thr)
+  if (!cmp_f64 || op < XC_OP_GT || op > XC_OP_NE) return (float)thr;
+  float f = 0.f;
+  dispatch_op(op, [&](auto OPC) -> int32_t {
+    f = fold_f64<decltype(OPC)::value>(thr);
+    return XC_OK;
+  });
   return f;
 }
 

@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <math.h>
+#include <string.h>
 
 #include "../../include/xclim_b200.h"
 
@@ -48,8 +49,8 @@ __device__ __forceinline__ float4 ld_stream4(const float* p) {
 }
 
 // ---- comparison against a scalar threshold ------------------------------------------------------
-// A float64 threshold compared with float32 data is folded on the host into an equivalent float32
-// threshold by directed rounding (see fold_threshold), so the device only ever compares in float32.
+// A float64 threshold compared with float32 data is folded into an equivalent float32 threshold by
+// directed rounding (see fold_f64), so the device only ever compares in float32.
 template <int OP>
 __device__ __forceinline__ bool cmp(float x, float t) {
   if constexpr (OP == XC_OP_GT) return x > t;
@@ -71,8 +72,41 @@ __device__ __forceinline__ bool cmpd(double x, double t) {
   return x != t;
 }
 
+// f with d added to its bit pattern: one float32 step away from zero (d = 1) or towards it (d = -1)
+__host__ __device__ __forceinline__ float add_to_bits(float f, int32_t d) {
+#ifdef __CUDA_ARCH__
+  return __int_as_float(__float_as_int(f) + d);
+#else
+  int32_t i;
+  memcpy(&i, &f, sizeof i);
+  i += d;
+  memcpy(&f, &i, sizeof f);
+  return f;
+#endif
+}
+
+// The float32 threshold with the truth table of the float64 threshold t: (x op fold_f64<OP>(t)) == ((double)x op t)
+// for every float32 x, NaN included, so that a float64 compare (numpy promotes float32 data against a float64
+// threshold) costs one float32 compare.  > and <= take the largest float32 <= t, >= and < the smallest float32 >= t;
+// == and != keep t when it is a float32 and take NaN otherwise (never equal, always different).  NaN stays NaN.
+template <int OP>
+__host__ __device__ __forceinline__ float fold_f64(double t) {
+  float f = (float)t;
+  if (t != t) return f;
+  if constexpr (OP == XC_OP_EQ || OP == XC_OP_NE) {
+    return (double)f == t ? f : NAN;
+  } else if constexpr (OP == XC_OP_GT || OP == XC_OP_LE) {  // largest float32 <= t
+    if ((double)f > t) f = add_to_bits(f, (f > 0.f) ? -1 : 1);
+    if (f == 0.f && t < 0.0) f = -1.401298464e-45f;
+  } else {                                                  // smallest float32 >= t
+    if ((double)f < t) f = add_to_bits(f, (f >= 0.f) ? 1 : -1);
+    if (f == 0.f && t > 0.0) f = 1.401298464e-45f;
+  }
+  return f;
+}
+
 // Host: float32 threshold t32 such that for every float32 x:  (x op t32)  ==  ((double)x op thr)
-// when cmp_f64 != 0, or (x op (float)thr) when cmp_f64 == 0 (numpy>=2 weak-scalar promotion).
+// when cmp_f64 != 0 (fold_f64), or (x op (float)thr) when cmp_f64 == 0 (numpy>=2 weak-scalar promotion).
 float fold_threshold(int32_t op, double thr, int32_t cmp_f64);
 
 // dispatch a runtime operator to a compile-time constant

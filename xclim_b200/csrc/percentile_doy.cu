@@ -486,22 +486,6 @@ percentile_doy_uniform_kernel(const float* __restrict__ x, int32_t T, int64_t C,
   }
 }
 
-// float32 threshold t32 with (x op t32) == ((double)x op t) for every float32 x (directed rounding)
-template <int OP>
-__device__ __forceinline__ float fold_thr(double t) {
-  float f = __double2float_rn(t);
-  if (t != t) return f;  // NaN threshold: every compare is False
-  if constexpr (OP == XC_OP_GT || OP == XC_OP_LE) {  // largest float32 <= t
-    if ((double)f > t) f = __int_as_float(__float_as_int(f) + ((f > 0.f) ? -1 : 1));
-    if (f == 0.f && t < 0.0) f = -1.401298464e-45f;
-  } else {                                           // smallest float32 >= t
-    if ((double)f < t) f = __int_as_float(__float_as_int(f) + ((f >= 0.f) ? 1 : -1));
-    if (f == 0.f && t > 0.0) f = 1.401298464e-45f;
-  }
-  return f;
-}
-
-
 // (A day-by-day window-5 kernel with the fused per-year count of the same series -- tx90p sub-case 3a in one
 // pass -- was slower than the two-kernel path and was removed.)
 // Window 5, days handled in PAIRS.  With B(d) = Y(d-2..d+1) = A(d-1) U A(d+1) the windows of two
@@ -843,109 +827,8 @@ doy_interp_kernel(const double* __restrict__ tab, int32_t n_src, int64_t C, int3
 }
 
 // ------------------------------------------------------------------------------------------------
-// percentile-threshold count
+// percentile-threshold count (other layouts: period_count_thr_kernel in period_stats.cu)
 // ------------------------------------------------------------------------------------------------
-template <int OP, bool VALID>
-__global__ void __launch_bounds__(kThreads)
-doy_count_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, const int32_t* __restrict__ poff,
-                 const int16_t* __restrict__ doy, const double* __restrict__ table,
-                 int32_t* __restrict__ out, int32_t* __restrict__ valid) {
-  // blockIdx.x = period (fastest): the blocks sharing a cell range run together and share the
-  // table rows through L2; blockIdx.y = cell block
-  const int p = blockIdx.x;
-  const int64_t c = ((int64_t)blockIdx.y * kThreads + threadIdx.x) * 2;
-  if (c >= C) return;
-  const bool two = (c + 1 < C);
-  const int t0 = poff[p], t1 = poff[p + 1];
-  int32_t n0 = 0, n1 = 0, v0 = 0, v1 = 0;
-  const float* col = x + c;
-  if (two && ((ldx & 1) == 0) && ((C & 1) == 0) && ((reinterpret_cast<uintptr_t>(x) & 7u) == 0) &&
-      ((reinterpret_cast<uintptr_t>(table) & 15u) == 0)) {
-#pragma unroll 4
-    for (int t = t0; t < t1; ++t) {
-      const int d = doy[t] - 1;
-      const float2 xv = *reinterpret_cast<const float2*>(col + (int64_t)t * ldx);
-      const double2 th = *reinterpret_cast<const double2*>(table + (int64_t)d * C + c);
-      n0 += cmpd<OP>((double)xv.x, th.x) ? 1 : 0;
-      n1 += cmpd<OP>((double)xv.y, th.y) ? 1 : 0;
-      if constexpr (VALID) {
-        v0 += (xv.x == xv.x) ? 1 : 0;
-        v1 += (xv.y == xv.y) ? 1 : 0;
-      }
-    }
-  } else {
-    for (int t = t0; t < t1; ++t) {
-      const int d = doy[t] - 1;
-      const float a = col[(int64_t)t * ldx];
-      n0 += cmpd<OP>((double)a, table[(int64_t)d * C + c]) ? 1 : 0;
-      if constexpr (VALID) v0 += (a == a) ? 1 : 0;
-      if (two) {
-        const float b = col[(int64_t)t * ldx + 1];
-        n1 += cmpd<OP>((double)b, table[(int64_t)d * C + c + 1]) ? 1 : 0;
-        if constexpr (VALID) v1 += (b == b) ? 1 : 0;
-      }
-    }
-  }
-  out[(int64_t)p * C + c] = n0;
-  if (two) out[(int64_t)p * C + c + 1] = n1;
-  if constexpr (VALID) {
-    valid[(int64_t)p * C + c] = v0;
-    if (two) valid[(int64_t)p * C + c + 1] = v1;
-  }
-}
-
-// Generic periods / calendars, 4 cells per thread: the float64 table entry of (doy[t], cell) is
-// folded to the float32 threshold with the same truth table (directed rounding, fold_thr) so that
-// the element test is one float32 compare; 4 steps (16 B of data + 32 B of table per thread each)
-// are in flight before any use.  The table rows are shared through L2 by the blocks of the same
-// cell range (blockIdx.x = period is the fastest index).  Operators >, <, >=, <= only.
-template <int OP, bool VALID>
-__global__ void __launch_bounds__(kThreads)
-doy_count4_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, const int32_t* __restrict__ poff,
-                  const int16_t* __restrict__ doy, const double* __restrict__ table,
-                  int32_t* __restrict__ out, int32_t* __restrict__ valid) {
-  const int p = blockIdx.x;
-  const int64_t c = ((int64_t)blockIdx.y * kThreads + threadIdx.x) * 4;
-  if (c >= C) return;
-  const int t0 = poff[p], t1 = poff[p + 1];
-  int32_t cn[4] = {0, 0, 0, 0}, vn[4] = {0, 0, 0, 0};
-  const float* col = x + c;
-  const double* trow = table + c;
-  constexpr int U = 4;
-  auto tally = [&](const float4& v, const double2& ta, const double2& tb) {
-    const float thr[4] = {fold_thr<OP>(ta.x), fold_thr<OP>(ta.y), fold_thr<OP>(tb.x), fold_thr<OP>(tb.y)};
-    const float xv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      cn[i] += cmp<OP>(xv[i], thr[i]) ? 1 : 0;
-      if constexpr (VALID) vn[i] += (xv[i] == xv[i]) ? 1 : 0;
-    }
-  };
-  int t = t0;
-  for (; t + U <= t1; t += U) {
-    float4 v[U];
-    double2 ta[U], tb[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int d = doy[t + u] - 1;
-      v[u] = ld_stream4(col + (int64_t)(t + u) * ldx);
-      ta[u] = *reinterpret_cast<const double2*>(trow + (int64_t)d * C);
-      tb[u] = *reinterpret_cast<const double2*>(trow + (int64_t)d * C + 2);
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) tally(v[u], ta[u], tb[u]);
-  }
-  for (; t < t1; ++t) {
-    const int d = doy[t] - 1;
-    const float4 v = ld_stream4(col + (int64_t)t * ldx);
-    const double2 ta = *reinterpret_cast<const double2*>(trow + (int64_t)d * C);
-    const double2 tb = *reinterpret_cast<const double2*>(trow + (int64_t)d * C + 2);
-    tally(v, ta, tb);
-  }
-  store_vec4(out + (int64_t)p * C + c, cn);
-  if constexpr (VALID) store_vec4(valid + (int64_t)p * C + c, vn);
-}
-
 // Year-blocked count for the common case "periods are whole years of equal length and the doy of a
 // step is its position in the year" (noleap / 360_day, freq YS): a thread owns 4 adjacent cells and
 // YB consecutive years, so every table row is fetched once per YB years instead of once per year
@@ -979,7 +862,7 @@ doy_count_years_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int6
       if (j < ny) v[j] = ld_stream4(base + (int64_t)j * ystride + (int64_t)d * ldx);
   };
   auto tally = [&](const double2& ta, const double2& tb, const float4 (&v)[YB]) {
-    const float thr[4] = {fold_thr<OP>(ta.x), fold_thr<OP>(ta.y), fold_thr<OP>(tb.x), fold_thr<OP>(tb.y)};
+    const float thr[4] = {fold_f64<OP>(ta.x), fold_f64<OP>(ta.y), fold_f64<OP>(tb.x), fold_f64<OP>(tb.y)};
 #pragma unroll
     for (int j = 0; j < YB; ++j) {
       if (j < ny) {
@@ -1376,53 +1259,6 @@ extern "C" int32_t xc_doy_interp_f64(const double* table, int32_t n_src, int64_t
   dim3 grid((unsigned)((C + 255) / 256), (unsigned)(n_out < 64 ? n_out : 64), 1);
   doy_interp_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(table, n_src, C, doy_min, doy_max, out);
   return launch_status("doy_interp_kernel");
-}
-
-extern "C" int32_t xc_doy_threshold_count_f32(const float* x, int64_t T, int64_t C, int64_t ldx,
-                                              const int32_t* period_offsets, int32_t P,
-                                              const int16_t* doy_index, const double* table, int32_t n_doy,
-                                              int32_t op, int32_t* out_count, int32_t* valid_count, void* stream) {
-  XC_REQUIRE(x && period_offsets && doy_index && table && out_count, "null pointer argument");
-  XC_REQUIRE(T > 0 && C > 0 && ldx >= C && P > 0 && n_doy > 0, "bad shape");
-  (void)n_doy;
-  cudaStream_t st = (cudaStream_t)stream;
-  // 4 cells per thread with float32-folded thresholds when the layout allows 128-bit accesses and the
-  // operator is an inequality
-  const bool vec4 = (C % 4 == 0) && (ldx % 4 == 0) && aligned16(x) && aligned16(table) && aligned16(out_count) &&
-                    (valid_count == nullptr || aligned16(valid_count)) && op >= XC_OP_GT && op <= XC_OP_LE;
-  if (vec4) {
-    const int64_t cb4 = (C / 4 + kThreads - 1) / kThreads;
-    XC_REQUIRE(cb4 <= 65535, "too many cells for one launch: tile the grid by latitude");
-    dim3 grid4((unsigned)P, (unsigned)cb4, 1);
-    return dispatch_op(op, [&](auto OPC) -> int32_t {
-      constexpr int OP = decltype(OPC)::value;
-      if constexpr (OP == XC_OP_EQ || OP == XC_OP_NE) {
-        return XC_ERR_INVALID;  // unreachable: vec4 requires an inequality
-      } else {
-        if (valid_count)
-          doy_count4_kernel<OP, true><<<grid4, kThreads, 0, st>>>(x, C, ldx, period_offsets, doy_index, table,
-                                                                  out_count, valid_count);
-        else
-          doy_count4_kernel<OP, false><<<grid4, kThreads, 0, st>>>(x, C, ldx, period_offsets, doy_index, table,
-                                                                   out_count, valid_count);
-        return launch_status("doy_count4_kernel");
-      }
-    });
-  }
-  const int64_t pairs = (C + 1) / 2;
-  const int64_t cblocks = (pairs + kThreads - 1) / kThreads;
-  XC_REQUIRE(cblocks <= 65535, "too many cells for one launch: tile the grid by latitude");
-  dim3 grid((unsigned)P, (unsigned)cblocks, 1);
-  return dispatch_op(op, [&](auto OPC) -> int32_t {
-    constexpr int OP = decltype(OPC)::value;
-    if (valid_count)
-      doy_count_kernel<OP, true><<<grid, kThreads, 0, st>>>(x, C, ldx, period_offsets, doy_index, table, out_count,
-                                                            valid_count);
-    else
-      doy_count_kernel<OP, false><<<grid, kThreads, 0, st>>>(x, C, ldx, period_offsets, doy_index, table, out_count,
-                                                             valid_count);
-    return launch_status("doy_count_kernel");
-  });
 }
 
 extern "C" int32_t xc_doy_threshold_count_years_f32(const float* x, int64_t T, int64_t C, int64_t ldx,

@@ -367,30 +367,95 @@ int32_t check_common(const void* x, int64_t T, int64_t C, int64_t ldx, const voi
 
 
 // ------------------------------------------------------------------------------------------------
-// threshold count against an ARRAY threshold (indices/generic.py:301-361 with a DataArray threshold:
-// numpy compares float32 data with a float64 array in float64, SURVEY.md A.1); thr_tstride = 0 for a
-// per-cell threshold (lat, lon), C for one that also varies in time.
+// threshold count against a float64 threshold that varies by cell: a day-of-year table (indices/_multivariate.py:
+// 1583-1590, `tx90p` & family, with `resample_doy` as an index into the table) or an array (indices/generic.py:
+// 301-361 with a DataArray threshold).  numpy compares float32 data with a float64 threshold in float64 (SURVEY.md
+// A.1); each threshold is folded to the float32 one with the same truth table (fold_f64), so that the element test
+// is one float32 compare.
+//   out[p, c] = #{ t in p : x[t, c] op thr[row(t) * rstride + c] },  row(t) = doy[t] - 1, or t without doy
+// (rstride = 0: one threshold per cell).  The grid is (period, cell block) with the period fastest, so that the
+// blocks of one cell range run together and share the threshold rows through L2.  U steps of data and thresholds
+// are in flight before any use.
 // ------------------------------------------------------------------------------------------------
-template <int OP>
-__global__ void __launch_bounds__(kThreads)
-period_count_arr_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, const int32_t* __restrict__ poff,
-                        const double* __restrict__ thr, int64_t thr_tstride, int32_t* __restrict__ out) {
-  const int64_t c = (int64_t)blockIdx.x * kThreads + threadIdx.x;
-  if (c >= C) return;
-  const int p = blockIdx.y;
-  const int t0 = poff[p], t1 = poff[p + 1];
-  int32_t n = 0;
-  const float* px = x + (int64_t)t0 * ldx + c;
-  const double* pt = thr + (int64_t)t0 * thr_tstride + c;
-#pragma unroll 4
-  for (int t = t0; t < t1; ++t) {
-    n += cmpd<OP>((double)ld_stream(px), *pt) ? 1 : 0;
-    px += ldx;
-    pt += thr_tstride;
+template <int VEC>
+__device__ __forceinline__ void load_thr(const double* p, double (&t)[VEC]) {
+  if constexpr (VEC == 4) {
+    const double2 a = *reinterpret_cast<const double2*>(p), b = *reinterpret_cast<const double2*>(p + 2);
+    t[0] = a.x; t[1] = a.y; t[2] = b.x; t[3] = b.y;
+  } else {
+    t[0] = *p;
   }
-  out[(int64_t)p * C + c] = n;
 }
 
+template <int OP, int VEC, bool VALID, bool DOY>
+__global__ void __launch_bounds__(kThreads)
+period_count_thr_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, const int32_t* __restrict__ poff,
+                        const int16_t* __restrict__ doy, const double* __restrict__ thr, int64_t rstride,
+                        int32_t* __restrict__ out, int32_t* __restrict__ valid) {
+  constexpr int U = 4;
+  const int p = blockIdx.x;
+  const int64_t c0 = ((int64_t)blockIdx.y * kThreads + threadIdx.x) * VEC;
+  if (c0 >= C) return;
+  const int t0 = poff[p], t1 = poff[p + 1];
+  int32_t cnt[VEC], nv[VEC];
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) { cnt[i] = 0; nv[i] = 0; }
+  const float* col = x + c0;
+  const double* tcol = thr + c0;
+  auto load = [&](int t, Vec<VEC>& r, double (&th)[VEC]) {
+    r.load(col + (int64_t)t * ldx);
+    load_thr<VEC>(tcol + (DOY ? (int64_t)(doy[t] - 1) : (int64_t)t) * rstride, th);
+  };
+  auto tally = [&](const Vec<VEC>& r, const double (&th)[VEC]) {
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) {
+      cnt[i] += cmp<OP>(r.v[i], fold_f64<OP>(th[i])) ? 1 : 0;
+      if constexpr (VALID) nv[i] += (r.v[i] == r.v[i]) ? 1 : 0;
+    }
+  };
+  int t = t0;
+  for (; t + U <= t1; t += U) {
+    Vec<VEC> r[U];
+    double th[U][VEC];
+#pragma unroll
+    for (int u = 0; u < U; ++u) load(t + u, r[u], th[u]);
+#pragma unroll
+    for (int u = 0; u < U; ++u) tally(r[u], th[u]);
+  }
+  for (; t < t1; ++t) {
+    Vec<VEC> r;
+    double th[VEC];
+    load(t, r, th);
+    tally(r, th);
+  }
+  store_vec<VEC>(out + (int64_t)p * C + c0, cnt);
+  if constexpr (VALID) store_vec<VEC>(valid + (int64_t)p * C + c0, nv);
+}
+
+// 4 cells per thread when the layout allows 128-bit accesses, 1 otherwise; valid counts with a doy index only
+template <bool DOY>
+int32_t launch_count_thr(const float* x, int64_t C, int64_t ldx, const int32_t* poff, int32_t P, const int16_t* doy,
+                         const double* thr, int64_t rstride, int32_t op, int32_t* out, int32_t* valid, cudaStream_t st) {
+  const bool v4 = can_vec4(x, C, ldx, out, valid) && aligned16(thr) && rstride % 4 == 0;
+  return dispatch_op(op, [&](auto OPC) -> int32_t {
+    auto go = [&](auto VECC, auto VALC) -> int32_t {
+      constexpr int VEC = decltype(VECC)::value;
+      const int64_t cblocks = (C + VEC * kThreads - 1) / (VEC * kThreads);
+      XC_REQUIRE(cblocks <= 65535, "too many cells for one launch: tile the grid by latitude");
+      const dim3 grid((unsigned)P, (unsigned)cblocks, 1);
+      period_count_thr_kernel<decltype(OPC)::value, VEC, decltype(VALC)::value, DOY><<<grid, kThreads, 0, st>>>(
+          x, C, ldx, poff, doy, thr, rstride, out, valid);
+      return launch_status("period_count_thr_kernel");
+    };
+    auto go2 = [&](auto VECC) -> int32_t {
+      if constexpr (DOY) {
+        if (valid) return go(VECC, std::true_type{});
+      }
+      return go(VECC, std::false_type{});
+    };
+    return v4 ? go2(std::integral_constant<int, 4>{}) : go2(std::integral_constant<int, 1>{});
+  });
+}
 
 // ------------------------------------------------------------------------------------------------
 // fused multi-output pass: every count / run statistic / reduction that shares (x, periods)
@@ -809,11 +874,16 @@ extern "C" int32_t xc_period_count_arr_f32(const float* x, int64_t T, int64_t C,
   if (e) return e;
   XC_REQUIRE(thr != nullptr, "null pointer argument");
   XC_REQUIRE(thr_tstride == 0 || thr_tstride >= C, "threshold time stride must be 0 (per cell) or >= C");
-  cudaStream_t st = (cudaStream_t)stream;
-  dim3 grid((unsigned)((C + kThreads - 1) / kThreads), (unsigned)P, 1);
-  return dispatch_op(op, [&](auto OPC) -> int32_t {
-    constexpr int OP = decltype(OPC)::value;
-    period_count_arr_kernel<OP><<<grid, kThreads, 0, st>>>(x, C, ldx, period_offsets, thr, thr_tstride, out_count);
-    return launch_status("period_count_arr_kernel");
-  });
+  return launch_count_thr<false>(x, C, ldx, period_offsets, P, nullptr, thr, thr_tstride, op, out_count, nullptr,
+                                 (cudaStream_t)stream);
+}
+
+extern "C" int32_t xc_doy_threshold_count_f32(const float* x, int64_t T, int64_t C, int64_t ldx,
+                                              const int32_t* period_offsets, int32_t P,
+                                              const int16_t* doy_index, const double* table, int32_t n_doy,
+                                              int32_t op, int32_t* out_count, int32_t* valid_count, void* stream) {
+  XC_REQUIRE(x && period_offsets && doy_index && table && out_count, "null pointer argument");
+  XC_REQUIRE(T > 0 && C > 0 && ldx >= C && P > 0 && n_doy > 0, "bad shape");
+  return launch_count_thr<true>(x, C, ldx, period_offsets, P, doy_index, table, C, op, out_count, valid_count,
+                                (cudaStream_t)stream);
 }

@@ -43,28 +43,42 @@ def dry_days(pr, thresh="0.2 mm/d", freq="YS", op="<"):
 
 
 # ------------------------------------------------------------------ percentile-threshold day counts
-def _percentile_day_count(da, per, freq, bootstrap, op, constrain):
-    """Shared body of tx90p & family -- indices/_multivariate.py:1583-1590:
-    ``thresh = resample_doy(per, da); threshold_count(da, op, thresh, freq)``; the (lat, lon, time)
-    float64 threshold array of the reference is never built: the kernel indexes the per-doy table."""
+def _percentile_day_count(da, per, freq, bootstrap, op, constrain, floor=None):
+    """Shared body of tx90p & family -- indices/_multivariate.py:1583-1590 (``floor``: _percentile_table_count)."""
     import numpy as np
 
-    from . import _lib, device
-    from .calendar import adjust_table, table_on_device
-    from .generic import _unwrap, _wrap_periods
+    from . import _lib
+    from .generic import _wrap_periods
     from .field import attrs_of
 
     code = _lib.op_code(op, constrain)
     if bootstrap:
         from .bootstrapping import bootstrap_doy_count
         return bootstrap_doy_count(da, per, freq, op, constrain)
-    x2d, cell_shape, other, ta = _unwrap(da)
-    table = _table_in_units_of(table_on_device(per, cell_shape, other, x2d.device), per, da)
-    table, doy_idx = adjust_table(table, ta)
-    out, _ = device.doy_threshold_count(x2d, ta.period_offsets(freq), doy_idx, table, code)
+    out, _, (cell_shape, other, ta) = _percentile_table_count(da, per, code, freq, floor)
     attrs = attrs_of(da)
     attrs["units"] = "d"
     return _wrap_periods(da, out, cell_shape, other, ta, freq, attrs, dtype=np.int64)
+
+
+def _percentile_table_count(da, per, code, freq, floor=None, want_valid=False):
+    """``thresh = resample_doy(per, da); threshold_count(da, op, thresh, freq)`` (indices/_multivariate.py:1583-1590)
+    without the (lat, lon, time) float64 threshold array of the reference: the kernel indexes the per-doy table,
+    converted to ``da``'s units and, with ``floor``, raised to ``floor`` where it is lower or NaN.  Returns the
+    counts, the valid (non-NaN) counts when ``want_valid`` (else None) and ``(cell_shape, other, ta)`` of ``da``."""
+    import torch
+
+    from . import device
+    from .calendar import adjust_table, table_on_device
+    from .generic import _unwrap
+
+    x2d, cell_shape, other, ta = _unwrap(da)
+    table = _table_in_units_of(table_on_device(per, cell_shape, other, x2d.device), per, da)
+    if floor is not None:
+        table = torch.where(table > floor, table, torch.full_like(table, floor))
+    table, doy_idx = adjust_table(table, ta)
+    cnt, valid = device.doy_threshold_count(x2d, ta.period_offsets(freq), doy_idx, table, code, want_valid=want_valid)
+    return cnt, valid, (cell_shape, other, ta)
 
 
 def _table_in_units_of(table, per, da):
@@ -85,26 +99,10 @@ def days_over_precip_thresh(pr, pr_per, thresh="1 mm/day", freq="YS", bootstrap=
     """Days with precipitation over both a doy percentile and a wet-day threshold (ETCCDI R95p-days) --
     indices/_multivariate.py:1176-1233: ``tp = pr_per.where(pr_per > thresh, thresh)`` then the tx90p
     count; the clamp is applied to the per-doy table on the device."""
-    import numpy as np
-    import torch
-
-    from . import _lib, device
-    from .calendar import adjust_table, table_on_device
-    from .field import attrs_of
-    from .generic import _unwrap, _wrap_periods
-
     if bootstrap:
         raise NotImplementedError("days_over_precip_thresh(bootstrap=True) is not supported by the xclim_b200 hot path")
-    code = _lib.op_code(op, (">", ">="))
     thr = threshold_in_units_of(thresh, pr) if isinstance(thresh, str) else float(thresh)
-    x2d, cell_shape, other, ta = _unwrap(pr)
-    table = _table_in_units_of(table_on_device(pr_per, cell_shape, other, x2d.device), pr_per, pr)
-    table = torch.where(table > thr, table, torch.full_like(table, thr))     # NaN percentiles -> thresh
-    table, doy_idx = adjust_table(table, ta)
-    out, _ = device.doy_threshold_count(x2d, ta.period_offsets(freq), doy_idx, table, code)
-    attrs = attrs_of(pr)
-    attrs["units"] = "d"
-    return _wrap_periods(pr, out, cell_shape, other, ta, freq, attrs, dtype=np.int64)
+    return _percentile_day_count(pr, pr_per, freq, False, op, (">", ">="), floor=thr)
 
 
 def tx90p(tasmax, tasmax_per, freq="YS", bootstrap=False, op=">"):
