@@ -344,6 +344,50 @@ def main():
                 dt = time.perf_counter() - t0
                 extra["cpu_port"] = {"cells_per_s": Sf / dt, "cores": 1, "kind": "port", "sample": f"({T}, {Sf}) cells, {dt:.1f} s"}
             report(label, ms, (n_in + n_out) * T * C * 4 + (T * C if "season_mask" in outs else 0), extra)
+    if want("ens") and a.only:      # ensemble statistics: opt-in (--only ens), on their own full-grid inputs
+        import subprocess
+
+        from oracle import ensemble_oracle as EO
+        del tas, pr
+        torch.cuda.empty_cache()
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True)
+        card = {"gpu": torch.cuda.get_device_name(), "power_limit": q.stdout.strip() or "unknown"}
+        g = torch.Generator(device="cuda").manual_seed(5)
+        years, grid = 150, 721 * 1440
+        per = [10, 50, 90]
+        # an annual indicator of R members over 150 years on the full grid, then R = 100 on a band that fits
+        for R, rows in ((30, 721), (100, 180)):
+            N = years * rows * 1440
+            x = torch.randn((R, N), generator=g, device="cuda", dtype=torch.float32).mul_(3.0).add_(285.0)
+            out = device.ens_percentiles(x, per, 1.0, 1.0, 1)
+            ms = timeit(lambda: device.ens_percentiles(x, per, 1.0, 1.0, 1), a.steps)
+            cols = np.r_[np.arange(0, N, max(1, N // 509)), N - 1]
+            got = out[:, cols].cpu().numpy()
+            exp = EO.percentiles(x[:, cols].cpu().numpy(), per)
+            report(f"ens_percentiles R={R} (10, 50, 90), {years} years x {rows} x 1440", ms, R * N * 4 + len(per) * N * 8,
+                   {"columns": N, "path": "registers" if R <= 32 else "shared memory",
+                    "oracle_check": {"cells": int(cols.size), "bit_equal": bool(np.array_equal(got, exp))}, **card})
+            del x, out
+            torch.cuda.empty_cache()
+        R, Ty = 30, 30
+        fut = torch.randn((R, Ty, grid), generator=g, device="cuda", dtype=torch.float32).add_(0.3)
+        ref = torch.randn((R, Ty, grid), generator=g, device="cuda", dtype=torch.float32)
+        code = _lib.ENS_TESTS["ttest"]
+        frac, pv = device.ens_robustness(fut, ref, None, code, 0.05, True, True)
+        ms = timeit(lambda: device.ens_robustness(fut, ref, None, code, 0.05, True, True), a.steps)
+        cols = np.r_[np.arange(0, grid, grid // 127), grid - 1]
+        exp, p, _ = EO.robustness(fut[:, :, cols].cpu().numpy(), ref[:, :, cols].cpu().numpy(), "ttest")
+        fr = frac[:, cols].cpu().numpy()
+        pk = pv[:, cols].cpu().numpy()
+        pos = p > 0                                   # p = 0 (t = +-inf) has no relative difference
+        check = {"cells": int(cols.size),
+                 "fractions_equal": bool(all(np.array_equal(fr[k], exp[n]) for k, n in enumerate(EO.FRACTIONS))),
+                 "pvals_zero_and_nan_equal": bool(np.array_equal(pk == 0, p == 0)
+                                                  and np.array_equal(np.isnan(pk), np.isnan(p))),
+                 "max_pval_rel_diff_f32": float(np.max(np.abs(pk[pos] - p[pos]) / p[pos])) if pos.any() else 0.0}
+        report(f"ens_robustness ttest R={R}, {Ty} + {Ty} years x 721 x 1440", ms, 2 * R * Ty * grid * 4 + 7 * grid * 8
+               + R * grid * 4, {"cells": grid, "oracle_check": check, **card})
 
 
 if __name__ == "__main__":

@@ -619,6 +619,53 @@ int32_t xc_si_apply_f32(const float* x, int64_t T, int64_t C, int64_t ldx, const
                         int32_t dist, int32_t zero_inflated, double interp, double alpha, double beta, double* out,
                         int64_t ldo, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * e1  Ensemble statistics across realizations -- ensembles/_base.py, ensembles/_robustness.py
+ *   The ensemble is an (R, N) matrix of N independent columns, x[r * ldr + n] (device float32, ldr >= N: a lat
+ *   tile of a wider buffer is a column range with the buffer's member stride).  1 <= R <= XC_ENS_MAX_MEMBERS.
+ * ------------------------------------------------------------------------------------------- */
+#define XC_ENS_MAX_MEMBERS 128
+/* The percentiles (host array of n_per <= 32 values in [0, 100]) of each column's non-NaN values, by the
+ * Hyndman-Fan (alpha, beta) plotting position: `ensemble_percentiles` (_base.py:329-342) = `calc_perc`
+ * (core/utils.py:279-323) along realization, `_nan_quantile` (:494-557) bit for bit, then the
+ * `min_members` mask (_base.py:356-357): NaN where fewer than min_members values are not NaN.  out is (n_per, N)
+ * float64 for R >= 2 and float32 for R == 1 (the np.take branch, :515-517). */
+int32_t xc_ens_percentiles_f32(const float* x, int64_t R, int64_t N, int64_t ldr, const double* percentiles,
+                               int32_t n_per, double alpha, double beta, int32_t min_members, void* out,
+                               void* stream);
+/* Mean, standard deviation (ddof 0), minimum and maximum of each column's non-NaN values, NaN where fewer than
+ * min_members (and no) values are not NaN: `ensemble_mean_std_max_min` (_base.py:178-206).  weights == NULL:
+ * mean / std float32 (N), float64 sums in member order rounded once; weights (device float64, R): xarray's
+ * Weighted.mean / .std, float64 (N), NaN where the weights of the valid members sum to 0.  vmin / vmax float32. */
+int32_t xc_ens_moments_f32(const float* x, int64_t R, int64_t N, int64_t ldr, const double* weights,
+                           int32_t min_members, void* mean, void* std, float* vmin, float* vmax, void* stream);
+/* `robustness_fractions` (_robustness.py:74-333) per cell: fut (R, Tf, C) at fut[r * ldf_r + t * ldf_t + c],
+ * ref (R, Tr, C) likewise or NULL (fut then holds deltas, Tf = 1).  A member is valid when none of its fut and
+ * ref values is NaN (MissingAny); its delta is the difference of the float64 NaN-omitting means.  `changed`:
+ *   XC_ENS_TEST_NONE   always                                 (:229-232)
+ *   XC_ENS_TEST_ABS    |delta| > param                        (:237)
+ *   XC_ENS_TEST_REL    |delta / mean(ref)| > param            (:240)
+ *   XC_ENS_TEST_TTEST  p < param, ttest_1samp(fut, mean(ref)) (:518-549)
+ *   XC_ENS_TEST_WELCH  p < param, Welch's t-test              (:552-581)
+ *   XC_ENS_TEST_IPCC   |delta| > sqrt(2/20) 1.645 sigma        (:636-661, without ref_pi), sigma the std of the
+ *                      residuals of the float64 least-squares line through the member's annual means of ref,
+ *                      ref_annual (R, P, C) at ref_annual[r * lda_r + p * C + c] (float32, from xc_period_reduce_f32
+ *                      with YS periods), against ys_time[P] (device float64: the YS timestamps, e.g. in days)
+ * with float64 p-values (ensemble_core.cuh).  ref_annual / ys_time are NULL for the other tests.  fractions (7, C) float64: changed, positive, changed_positive,
+ * negative, changed_negative, valid, agree, as :257-271 with weights (device float64, R, or NULL for ones) and
+ * strict_sign, NaN filled with 0 (:319).  pvals (R, C) float32 (t-tests only, or NULL). */
+#define XC_ENS_TEST_NONE  0
+#define XC_ENS_TEST_ABS   1
+#define XC_ENS_TEST_REL   2
+#define XC_ENS_TEST_TTEST 3
+#define XC_ENS_TEST_WELCH 4
+#define XC_ENS_TEST_IPCC  5
+int32_t xc_ens_robustness_f32(const float* fut, int64_t Tf, int64_t ldf_r, int64_t ldf_t, const float* ref,
+                              int64_t Tr, int64_t ldr_r, int64_t ldr_t, const float* ref_annual, int64_t P,
+                              int64_t lda_r, const double* ys_time, int64_t R, int64_t C,
+                              const double* weights, int32_t test, double param, int32_t strict_sign,
+                              double* fractions, float* pvals, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

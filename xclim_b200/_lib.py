@@ -83,7 +83,16 @@ SIGNATURES = {
                              _vp, _i64, _vp]),
     "xc_si_apply_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _f64, _f64, _f64, _vp,
                                _i64, _vp]),
+    "xc_ens_percentiles_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _f64, _f64, _i32, _vp, _vp]),
+    "xc_ens_moments_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "xc_ens_robustness_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64,
+                                     _vp, _i32, _f64, _i32, _vp, _vp, _vp]),
 }
+
+# ensembles (include/xclim_b200.h e1)
+ENS_MAX_MEMBERS, ENS_MAX_PER = 128, 32
+ENS_TESTS = {None: 0, "abs_thresh": 1, "rel_thresh": 2, "ttest": 3, "welch-ttest": 4, "ipcc-ar6-c": 5}
+ENS_FRACTIONS = ("changed", "positive", "changed_positive", "negative", "changed_negative", "valid", "agree")
 
 # standardized indices (include/xclim_b200.h s1)
 SI_DISTS = {"gamma": 0, "fisk": 1, "lognorm": 2}

@@ -21,7 +21,7 @@
 
 #if defined(__CUDACC__)
 #define XC_SI_HD __host__ __device__ __forceinline__
-#define XC_SI_HDN __host__ __device__ __noinline__
+#define XC_SI_HDN static __host__ __device__ __noinline__   // static: ensemble_core.cuh includes this header too
 #else
 #define XC_SI_HD inline
 #define XC_SI_HDN inline

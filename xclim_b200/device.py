@@ -609,6 +609,59 @@ def si_apply(x2d, group_of_step, params, n_zeros, n_notnull, dist_code, interp=1
     return out
 
 
+# ------------------------------------------------------------------------------------ ensembles
+def ens_percentiles(x2d, percentiles, alpha, beta, min_members):
+    """Percentiles along the member axis of an (R, N) float32 matrix (xc_ens_percentiles_f32; column views with
+    a row stride > N work in place).  Returns (n_per, N): float64 for R >= 2, float32 for R == 1."""
+    R, N = x2d.shape
+    assert x2d.dtype == torch.float32 and x2d.stride(1) == 1
+    per = np.ascontiguousarray(np.asarray(percentiles, dtype=np.float64).ravel())
+    out = torch.empty((per.size, N), dtype=torch.float64 if R >= 2 else torch.float32, device=x2d.device)
+    for p0 in range(0, per.size, _lib.ENS_MAX_PER):
+        chunk = per[p0:p0 + _lib.ENS_MAX_PER]
+        check(load().xc_ens_percentiles_f32(x2d.data_ptr(), R, N, x2d.stride(0), chunk.ctypes.data, chunk.size,
+                                            float(alpha), float(beta), int(min_members), out[p0].data_ptr(),
+                                            current_stream_ptr()))
+    return out
+
+
+def ens_moments(x2d, weights, min_members):
+    """(mean, std, min, max) along the member axis of an (R, N) float32 matrix (xc_ens_moments_f32): mean / std
+    float32 without weights, float64 with ``weights`` (a float64 device tensor of R values)."""
+    R, N = x2d.shape
+    assert x2d.dtype == torch.float32 and x2d.stride(1) == 1
+    dt = torch.float32 if weights is None else torch.float64
+    mean, std = (torch.empty(N, dtype=dt, device=x2d.device) for _ in range(2))
+    vmin, vmax = (torch.empty(N, dtype=torch.float32, device=x2d.device) for _ in range(2))
+    check(load().xc_ens_moments_f32(x2d.data_ptr(), R, N, x2d.stride(0), _ptr(weights), int(min_members),
+                                    mean.data_ptr(), std.data_ptr(), vmin.data_ptr(), vmax.data_ptr(),
+                                    current_stream_ptr()))
+    return mean, std, vmin, vmax
+
+
+def ens_robustness(fut, ref, weights, test_code, param, strict_sign, want_pvals, ref_annual=None, ys_time=None):
+    """Robustness fractions (7, C) float64 and the (R, C) float32 p-values (or None) of ``fut`` / ``ref`` given as
+    (R, T, C) float32 device tensors with unit cell stride (``ref`` None: ``fut`` is (R, 1, C) deltas).  ipcc-ar6-c
+    also takes ``ref_annual`` (R, P, C) float32 (the YS means of ``ref``) and ``ys_time`` (P) float64 device
+    tensors."""
+    R, Tf, C = fut.shape
+    assert fut.dtype == torch.float32 and fut.stride(2) == 1
+    if ref is not None:
+        assert ref.dtype == torch.float32 and ref.stride(2) == 1 and ref.shape[0] == R and ref.shape[2] == C
+    frac = torch.empty((7, C), dtype=torch.float64, device=fut.device)
+    pvals = torch.empty((R, C), dtype=torch.float32, device=fut.device) if want_pvals else None
+    Tr, sr_r, sr_t = (ref.shape[1], ref.stride(0), ref.stride(1)) if ref is not None else (0, 0, 0)
+    P, sa_r = 0, 0
+    if ref_annual is not None:
+        assert ref_annual.dtype == torch.float32 and ref_annual.stride(2) == 1 and ref_annual.stride(1) == C
+        assert ys_time.dtype == torch.float64 and ys_time.is_contiguous() and ys_time.numel() == ref_annual.shape[1]
+        P, sa_r = ref_annual.shape[1], ref_annual.stride(0)
+    check(load().xc_ens_robustness_f32(fut.data_ptr(), Tf, fut.stride(0), fut.stride(1), _ptr(ref), Tr, sr_r, sr_t,
+                                       _ptr(ref_annual), P, sa_r, _ptr(ys_time), R, C, _ptr(weights), int(test_code), float(param), int(bool(strict_sign)),
+                                       frac.data_ptr(), _ptr(pvals), current_stream_ptr()))
+    return frac, pvals
+
+
 # ------------------------------------------------------------------------------------ fire weather
 FWI_OUTPUTS = ("DC", "DMC", "FFMC", "ISI", "BUI", "FWI", "DSR")
 
