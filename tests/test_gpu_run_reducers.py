@@ -87,6 +87,22 @@ def test_period_runstat_vec4_vec1(cuda, window, before):
             _same_bits(got, msg)
 
 
+# ----------------------------------------------------------------------------------------- period_run_maxsum_kernel
+@pytest.mark.parametrize("window", [1, 3])
+@pytest.mark.parametrize("before", [True, False])
+def test_period_run_maxsum_vec4_vec1(cuda, window, before):
+    from xclim_b200 import _lib, device
+    x = _field(11)
+    views = _views(x)
+    for op in (">", "<"):
+        args = (POFF, _lib.OPS[op], THR, window, before)
+        exp = F.period_run_maxsum(x, *args).numpy()
+        got = [device.period_run_maxsum(v, *args).cpu().numpy() for v in views]
+        msg = f"{op} w={window} before={before}"
+        np.testing.assert_allclose(got[0], exp, rtol=1e-5, atol=1e-6, err_msg=msg)
+        _same_bits(got, msg)
+
+
 # --------------------------------------------------------------------- spell_sumw / spell_runstat4 / spell_runstat
 # (window statistic, window): aligned kernel / offset-slice kernel
 SPELL_CASES = [

@@ -46,11 +46,11 @@ period_runstat2_kernel(const float* __restrict__ x1, const float* __restrict__ x
   if (c0 >= C) return;
   const int p = blockIdx.y;
   const int t0 = poff[p], tend = poff[p + 1];
-  int cur[VEC];
-  bool skip[VEC];
+  int32_t cur[VEC];
+  PeriodMask pm[VEC];
   RunAcc<RED> acc[VEC];
 #pragma unroll
-  for (int i = 0; i < VEC; ++i) { cur[i] = 0; skip[i] = false; acc[i].init(); }
+  for (int i = 0; i < VEC; ++i) { cur[i] = 0; pm[i].init(); acc[i].init(); }
   auto cond = [&](float u, float v) -> bool {
     bool c1, c2;
     if constexpr (GTGT) {
@@ -62,78 +62,56 @@ period_runstat2_kernel(const float* __restrict__ x1, const float* __restrict__ x
     }
     return any ? (c1 | c2) : (c1 & c2);
   };
-  auto load = [&](const float* base, int t, float (&v)[VEC]) {
-    if constexpr (VEC == 4) {
-      const float4 q = ld_stream4(base + (int64_t)t * ldx + c0);
-      v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
-    } else {
-      v[0] = ld_stream(base + (int64_t)t * ldx + c0);
-    }
+  auto load = [&](int t, Vec<VEC>& u, Vec<VEC>& v) {
+    u.load(x1 + (int64_t)t * ldx + c0);
+    v.load(x2 + (int64_t)t * ldx + c0);
   };
   if (after && t0 > 0) {
-    float u[VEC], v[VEC];
-    load(x1, t0 - 1, u);
-    load(x2, t0 - 1, v);
+    Vec<VEC> u, v;
+    load(t0 - 1, u, v);
 #pragma unroll
-    for (int i = 0; i < VEC; ++i) skip[i] = cond(u[i], v[i]);
+    for (int i = 0; i < VEC; ++i) pm[i].look_back(cond(u.v[i], v.v[i]));
   }
-  auto step = [&](const float (&u)[VEC], const float (&v)[VEC], bool only_open) {
+  auto step = [&](const Vec<VEC>& u, const Vec<VEC>& v) {
 #pragma unroll
-    for (int i = 0; i < VEC; ++i) {
-      bool m = cond(u[i], v[i]);
-      if (after) {
-        if (only_open) {
-          m = m && (cur[i] > 0);
-        } else {
-          skip[i] = skip[i] && m;
-          m = m && !skip[i];
-        }
-      }
-      const int L = cur[i];
-      acc[i].add(L, !m && L >= window);
-      cur[i] = m ? L + 1 : 0;
-    }
+    for (int i = 0; i < VEC; ++i) run_step(cur[i], acc[i], pm[i].inside(after, cond(u.v[i], v.v[i])), window);
   };
   int t = t0;
   for (; t + kUnroll <= tend; t += kUnroll) {
-    float u[kUnroll][VEC], v[kUnroll][VEC];
+    Vec<VEC> u[kUnroll], v[kUnroll];
 #pragma unroll
-    for (int k = 0; k < kUnroll; ++k) { load(x1, t + k, u[k]); load(x2, t + k, v[k]); }
+    for (int k = 0; k < kUnroll; ++k) load(t + k, u[k], v[k]);
 #pragma unroll
-    for (int k = 0; k < kUnroll; ++k) step(u[k], v[k], false);
+    for (int k = 0; k < kUnroll; ++k) step(u[k], v[k]);
   }
   for (; t < tend; ++t) {
-    float u[VEC], v[VEC];
-    load(x1, t, u);
-    load(x2, t, v);
-    step(u, v, false);
+    Vec<VEC> u, v;
+    load(t, u, v);
+    step(u, v);
   }
   if (after) {
     bool open = false;
 #pragma unroll
     for (int i = 0; i < VEC; ++i) open = open || (cur[i] > 0);
-    while (open && t < (int)T) {
-      float u[VEC], v[VEC];
-      load(x1, t, u);
-      load(x2, t, v);
-      step(u, v, true);
+    for (; open && t < (int)T; ++t) {
+      Vec<VEC> u, v;
+      load(t, u, v);
       open = false;
 #pragma unroll
-      for (int i = 0; i < VEC; ++i) open = open || (cur[i] > 0);
-      ++t;
+      for (int i = 0; i < VEC; ++i) {
+        const bool m = PeriodMask::past_end(cond(u.v[i], v.v[i]), cur[i] > 0);
+        run_step(cur[i], acc[i], m, window);
+        open = open || m;
+      }
     }
   }
   float res[VEC];
 #pragma unroll
   for (int i = 0; i < VEC; ++i) {
-    acc[i].add(cur[i], cur[i] >= window);   // the run closed by the period / series end
+    run_close(cur[i], acc[i], window);
     res[i] = acc[i].result(reducer);
   }
-  if constexpr (VEC == 4) {
-    *reinterpret_cast<float4*>(out + (int64_t)p * C + c0) = make_float4(res[0], res[1], res[2], res[3]);
-  } else {
-    out[(int64_t)p * C + c0] = res[0];
-  }
+  store_vec<VEC>(out + (int64_t)p * C + c0, res);
 }
 
 }  // namespace

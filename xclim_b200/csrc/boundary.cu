@@ -9,7 +9,7 @@
 //                 period with da true on t..t+window-1 (the run may extend past the period end),
 //                 "last" = last t of the period with da true on t-window+1..t.
 // Output: float32 index relative to the period start, NaN when there is none.
-#include "common.cuh"
+#include "runstat.cuh"
 
 namespace xc {
 namespace {
@@ -251,8 +251,9 @@ run_quantile_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t l
   const int t0 = poff[p], t1 = poff[p + 1];
   const float* col = x + c;
   int m = 0, cur = 0, longest = 0;
-  bool skip = false;
-  if (after && t0 > 0) skip = cmp<OP>(ld_stream(col + (int64_t)(t0 - 1) * ldx), thr);
+  PeriodMask pm;
+  pm.init();
+  if (after && t0 > 0) pm.look_back(cmp<OP>(ld_stream(col + (int64_t)(t0 - 1) * ldx), thr));
   auto close_run = [&]() {   // a run that ends inside the period: cur <= t1 - t0 < 65536
     if (cur >= window && m < cap) {
       runs[(size_t)m++ * kThreads + lane] = (unsigned short)cur;
@@ -260,33 +261,15 @@ run_quantile_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t l
     }
     cur = 0;
   };
-  auto step = [&](float v) {
-    bool in = cmp<OP>(v, thr);
-    if (after) {
-      skip = skip && in;
-      in = in && !skip;
-    }
-    if (in) ++cur; else close_run();
-  };
-  {
-    constexpr int U = 8;      // rows in flight (the loop was one dependent load per step: 0.055 of the HBM roofline)
-    int t = t0;
-    const float* pp = col + (int64_t)t0 * ldx;
-    for (; t + U <= t1; t += U) {
-      float v[U];
-#pragma unroll
-      for (int u = 0; u < U; ++u) v[u] = ld_stream(pp + (int64_t)u * ldx);
-#pragma unroll
-      for (int u = 0; u < U; ++u) step(v[u]);
-      pp += (int64_t)U * ldx;
-    }
-    for (; t < t1; ++t) {
-      step(ld_stream(pp));
-      pp += ldx;
-    }
-  }
+  // 8 rows in flight (one dependent load per step reached 0.055 of the HBM roofline)
+  stream_rows<1, 8>(col, ldx, t0, t1, [&](const Vec<1>& r) {
+    if (pm.inside(after, cmp<OP>(r.v[0], thr))) ++cur; else close_run();
+  });
   if (after) {   // the run open at t1 belongs to this period with its full length
-    for (int t = t1; cur > 0 && t < (int)T && cmp<OP>(ld_stream(col + (int64_t)t * ldx), thr); ++t) ++cur;
+    for (int t = t1; cur > 0 && t < (int)T; ++t) {
+      if (!PeriodMask::past_end(cmp<OP>(ld_stream(col + (int64_t)t * ldx), thr), cur > 0)) break;
+      ++cur;
+    }
   }
   const int tail = cur >= window ? cur : 0;    // 0: no run
   longest = max(longest, tail);

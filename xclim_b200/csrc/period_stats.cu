@@ -26,60 +26,6 @@ namespace xc {
 namespace {
 
 constexpr int kThreads = 128;
-constexpr int kUnroll = 8;
-
-template <int VEC>
-struct Vec;
-template <>
-struct Vec<1> {
-  float v[1];
-  __device__ __forceinline__ void load(const float* p) { v[0] = ld_stream(p); }
-};
-template <>
-struct Vec<4> {
-  float v[4];
-  __device__ __forceinline__ void load(const float* p) {
-    float4 q = ld_stream4(p);
-    v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
-  }
-};
-
-template <int VEC, typename T>
-__device__ __forceinline__ void store_vec(T* dst, const T (&v)[VEC]) {
-  if constexpr (VEC == 4 && sizeof(T) == 4) {
-    uint4 q;
-    q.x = *reinterpret_cast<const uint32_t*>(&v[0]);
-    q.y = *reinterpret_cast<const uint32_t*>(&v[1]);
-    q.z = *reinterpret_cast<const uint32_t*>(&v[2]);
-    q.w = *reinterpret_cast<const uint32_t*>(&v[3]);
-    *reinterpret_cast<uint4*>(dst) = q;
-  } else {
-#pragma unroll
-    for (int i = 0; i < VEC; ++i) dst[i] = v[i];
-  }
-}
-
-// Iterate f(t, Vec) over t in [t0, t1) with UNROLL loads in flight.
-template <int VEC, int UNROLL = kUnroll, typename F>
-__device__ __forceinline__ void stream_rows(const float* __restrict__ col, int64_t ldx, int t0, int t1,
-                                            F&& f) {
-  int t = t0;
-  const float* p = col + (int64_t)t0 * ldx;
-  for (; t + UNROLL <= t1; t += UNROLL) {
-    Vec<VEC> r[UNROLL];
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) r[u].load(p + (int64_t)u * ldx);
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) f(r[u]);
-    p += (int64_t)UNROLL * ldx;
-  }
-  for (; t < t1; ++t) {
-    Vec<VEC> r;
-    r.load(p);
-    f(r);
-    p += ldx;
-  }
-}
 
 // ------------------------------------------------------------------------------------------------
 // threshold count (+ valid count)
@@ -110,8 +56,8 @@ period_count_kernel(const float* __restrict__ x, int64_t C, int64_t ldx,
 // ------------------------------------------------------------------------------------------------
 // run-length statistics
 // ------------------------------------------------------------------------------------------------
-// FASTMAX: reducer == max and window == 1 needs no run-end detection: max over t of the running
-// length (this is the maximum_consecutive_dry_days configuration).
+// FASTMAX: reducer == max and window == 1 takes run_step's running form, which needs no run-end detection
+// (this is the maximum_consecutive_dry_days configuration).
 template <int OP, int RED, int VEC, bool VALID, bool AFTER, bool FASTMAX>
 __global__ void __launch_bounds__(kThreads)
 period_runstat_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t ldx,
@@ -124,77 +70,50 @@ period_runstat_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t
   const float* col = x + c0;
 
   int32_t cur[VEC], nv[VEC];
-  bool skip[VEC];
+  PeriodMask pm[VEC];
   RunAcc<RED> acc[VEC];
 #pragma unroll
-  for (int i = 0; i < VEC; ++i) { cur[i] = 0; nv[i] = 0; skip[i] = false; acc[i].init(); }
+  for (int i = 0; i < VEC; ++i) { cur[i] = 0; nv[i] = 0; pm[i].init(); acc[i].init(); }
 
   if constexpr (AFTER) {
-    // A run already under way at the period start belongs to an earlier period
-    // (indices/run_length.py:329-334: run lengths sit on the run's FIRST element).
     if (t0 > 0) {
       Vec<VEC> r;
       r.load(col + (int64_t)(t0 - 1) * ldx);
 #pragma unroll
-      for (int i = 0; i < VEC; ++i) skip[i] = cmp<OP>(r.v[i], thr);
+      for (int i = 0; i < VEC; ++i) pm[i].look_back(cmp<OP>(r.v[i], thr));
     }
   }
 
-  auto step = [&](const Vec<VEC>& r) {
+  stream_rows<VEC>(col, ldx, t0, t1, [&](const Vec<VEC>& r) {
 #pragma unroll
     for (int i = 0; i < VEC; ++i) {
-      bool c = cmp<OP>(r.v[i], thr);
+      const bool c = cmp<OP>(r.v[i], thr);
       if constexpr (VALID) nv[i] += (r.v[i] == r.v[i]) ? 1 : 0;
-      if constexpr (AFTER) {
-        skip[i] = skip[i] && c;
-        c = c && !skip[i];
-      }
-      if constexpr (FASTMAX) {
-        cur[i] = c ? cur[i] + 1 : 0;
-        acc[i].a = max(acc[i].a, cur[i]);
-      } else {
-        const int32_t L = cur[i];
-        acc[i].add(L, !c && L >= window);
-        cur[i] = c ? L + 1 : 0;
-      }
+      run_step<FASTMAX>(cur[i], acc[i], pm[i].inside(AFTER, c), window);
     }
-  };
-  stream_rows<VEC>(col, ldx, t0, t1, step);
+  });
 
   if constexpr (AFTER) {
-    // Runs still open at the period end keep their FULL length: read on until they all close.
-    // (VALID counts only the period's own steps.)
-    int t = t1;
+    // read on until every open run has closed (VALID counts only the period's own steps)
     bool open = false;
 #pragma unroll
     for (int i = 0; i < VEC; ++i) open = open || (cur[i] > 0);
-    const float* pp = col + (int64_t)t1 * ldx;
-    while (open && t < (int)T) {
+    for (int t = t1; open && t < (int)T; ++t) {
       Vec<VEC> r;
-      r.load(pp);
+      r.load(col + (int64_t)t * ldx);
       open = false;
 #pragma unroll
       for (int i = 0; i < VEC; ++i) {
-        // a cell whose run has closed must not start a new one here (it belongs to a later period)
-        bool c = (cur[i] > 0) && cmp<OP>(r.v[i], thr);
-        if constexpr (FASTMAX) {
-          cur[i] = c ? cur[i] + 1 : 0;
-          acc[i].a = max(acc[i].a, cur[i]);
-        } else {
-          const int32_t L = cur[i];
-          acc[i].add(L, !c && L >= window);
-          cur[i] = c ? L + 1 : 0;
-        }
+        const bool c = PeriodMask::past_end(cmp<OP>(r.v[i], thr), cur[i] > 0);
+        run_step<FASTMAX>(cur[i], acc[i], c, window);
         open = open || c;
       }
-      pp += ldx;
-      ++t;
     }
   }
   float res[VEC];
 #pragma unroll
   for (int i = 0; i < VEC; ++i) {
-    if constexpr (!FASTMAX) acc[i].add(cur[i], cur[i] >= window);  // run closed by the period/series end
+    run_close<FASTMAX>(cur[i], acc[i], window);
     res[i] = acc[i].result();
   }
   store_vec<VEC>(out + (int64_t)p * C + c0, res);
@@ -218,9 +137,9 @@ period_run_maxsum_kernel(const float* __restrict__ x, int64_t T, int64_t C, int6
   const float* col = x + c0;
   int32_t cur[VEC];
   double rs[VEC], best[VEC];
-  bool skip[VEC];
+  PeriodMask pm[VEC];
 #pragma unroll
-  for (int i = 0; i < VEC; ++i) { cur[i] = 0; rs[i] = 0.0; best[i] = 0.0; skip[i] = false; }
+  for (int i = 0; i < VEC; ++i) { cur[i] = 0; rs[i] = 0.0; best[i] = 0.0; pm[i].init(); }
   auto excess = [&](float v) -> float {
     const float d = (OP == XC_OP_GT || OP == XC_OP_GE) ? (v - thr) : (thr - v);
     return (d > 0.f) ? d : 0.f;  // NaN -> 0: not part of a run (rle: da > 0)
@@ -230,46 +149,41 @@ period_run_maxsum_kernel(const float* __restrict__ x, int64_t T, int64_t C, int6
       Vec<VEC> r;
       r.load(col + (int64_t)(t0 - 1) * ldx);
 #pragma unroll
-      for (int i = 0; i < VEC; ++i) skip[i] = excess(r.v[i]) > 0.f;
+      for (int i = 0; i < VEC; ++i) pm[i].look_back(excess(r.v[i]) > 0.f);
     }
   }
-  auto step = [&](const Vec<VEC>& r, bool only_open) {
+  auto step = [&](int i, float e, bool in) {
+    if (in) {
+      cur[i] += 1;
+      rs[i] += (double)e;
+    } else {
+      if (cur[i] >= window) best[i] = fmax(best[i], rs[i]);
+      cur[i] = 0;
+      rs[i] = 0.0;
+    }
+  };
+  stream_rows<VEC>(col, ldx, t0, t1, [&](const Vec<VEC>& r) {
 #pragma unroll
     for (int i = 0; i < VEC; ++i) {
       const float e = excess(r.v[i]);
-      bool in = e > 0.f;
-      if constexpr (AFTER) {
-        if (!only_open) {
-          skip[i] = skip[i] && in;
-          in = in && !skip[i];
-        } else {
-          in = in && (cur[i] > 0);
-        }
-      }
-      if (in) {
-        cur[i] += 1;
-        rs[i] += (double)e;
-      } else {
-        if (cur[i] >= window) best[i] = fmax(best[i], rs[i]);
-        cur[i] = 0;
-        rs[i] = 0.0;
-      }
+      step(i, e, pm[i].inside(AFTER, e > 0.f));
     }
-  };
-  stream_rows<VEC>(col, ldx, t0, t1, [&](const Vec<VEC>& r) { step(r, false); });
+  });
   if constexpr (AFTER) {
-    int t = t1;
     bool open = false;
 #pragma unroll
     for (int i = 0; i < VEC; ++i) open = open || (cur[i] > 0);
-    while (open && t < (int)T) {
+    for (int t = t1; open && t < (int)T; ++t) {
       Vec<VEC> r;
       r.load(col + (int64_t)t * ldx);
-      step(r, true);
       open = false;
 #pragma unroll
-      for (int i = 0; i < VEC; ++i) open = open || (cur[i] > 0);
-      ++t;
+      for (int i = 0; i < VEC; ++i) {
+        const float e = excess(r.v[i]);
+        const bool in = PeriodMask::past_end(e > 0.f, cur[i] > 0);
+        step(i, e, in);
+        open = open || in;
+      }
     }
   }
   float res[VEC];
@@ -460,23 +374,13 @@ int32_t launch_count_thr(const float* x, int64_t C, int64_t ldx, const int32_t* 
 // ------------------------------------------------------------------------------------------------
 // fused multi-output pass: every count / run statistic / reduction that shares (x, periods)
 // ------------------------------------------------------------------------------------------------
-// One thread = 2 adjacent cells x one period (64-bit loads, kUnroll rows in flight); the state of NC
+// One thread = 2 adjacent cells x one period (64-bit loads, UNROLL rows in flight); the state of NC
 // conditions (run length, count, longest run), NR windowed run outputs, NM largest-run-sum outputs and NS
 // conditional sums lives in registers next to the plain statistics -- about 25 registers per cell for the
 // richest pass of the batch (tasmax), so that 4-5 CTAs stay resident per SM.  Per element and cell: 7
 // instructions per condition, 3 per run output, ~10 per run sum, 6 per conditional sum, 8 for the plain
 // statistics.  The template arguments are the (rounded-up) numbers of each kind: unused entries are
 // computed and dropped (their slots are -1).
-template <>
-struct Vec<2> {
-  float v[2];
-  __device__ __forceinline__ void load(const float* p) {
-    float2 q;
-    asm volatile("ld.global.nc.L1::no_allocate.v2.f32 {%0,%1}, [%2];" : "=f"(q.x), "=f"(q.y) : "l"(p));
-    v[0] = q.x; v[1] = q.y;
-  }
-};
-
 // a[j] for a warp-uniform runtime j without dynamic register indexing (which would go through local memory)
 template <int N, typename T>
 __device__ __forceinline__ T pick_uniform(const T (&a)[N], int j) {

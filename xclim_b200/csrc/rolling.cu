@@ -199,31 +199,17 @@ spell_runstat_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t 
     }
     return last_true >= 0 && last_true >= t - w + 1;
   };
-  bool skip = false;
-  if (after && t0 > 0) skip = mask_at(t0 - 1);  // a run already open belongs to an earlier period
-  int cur = 0;
+  PeriodMask pm;
+  pm.init();
+  if (after && t0 > 0) pm.look_back(mask_at(t0 - 1));
+  int32_t cur = 0;
   RunAcc<kRunAny> acc;
   acc.init();
-  auto step = [&](bool m) {
-    if (m) {
-      ++cur;
-    } else {
-      acc.add(cur, cur >= 1);
-      cur = 0;
-    }
-  };
-  for (int t = t0; t < t1; ++t) {
-    bool m = mask_at(t);
-    if (after) {
-      skip = skip && m;
-      m = m && !skip;
-    }
-    step(m);
-  }
+  for (int t = t0; t < t1; ++t) run_step(cur, acc, pm.inside(after, mask_at(t)), 1);
   if (after) {
-    for (int t = t1; cur > 0 && t < (int)T; ++t) step(mask_at(t));
+    for (int t = t1; cur > 0 && t < (int)T; ++t) run_step(cur, acc, PeriodMask::past_end(mask_at(t), cur > 0), 1);
   }
-  acc.add(cur, cur >= 1);
+  run_close(cur, acc, 1);
   out[(int64_t)p * C + c] = acc.result(reducer);
 }
 
@@ -367,28 +353,16 @@ spell_runstat4_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t
   const float* col = x + c;
   const int first_t = (AFTER && t0 > 0) ? t0 - 1 : t0;
   int last[4] = {-1, -1, -1, -1};
-  bool skip[4] = {false, false, false, false};
-  int cur[4] = {0, 0, 0, 0};
+  int32_t cur[4] = {0, 0, 0, 0};
+  PeriodMask pm[4];
   RunAcc<kRunAny> acc[4];
 #pragma unroll
-  for (int j = 0; j < 4; ++j) acc[j].init();
+  for (int j = 0; j < 4; ++j) { pm[j].init(); acc[j].init(); }
   // mask value of step t for cell j (t >= first_t, in time order)
   auto feed = [&](int j, int t, bool mk) {
-    if (AFTER) {
-      if (t < t0) { skip[j] = mk; return; }  // a run already open belongs to an earlier period
-      if (t < t1) {
-        skip[j] = skip[j] && mk;
-        mk = mk && !skip[j];
-      } else if (cur[j] == 0) {
-        return;                              // past the period end only an open run is followed
-      }
-    }
-    if (mk) {
-      ++cur[j];
-    } else {
-      acc[j].add(cur[j], cur[j] >= 1);
-      cur[j] = 0;
-    }
+    if (AFTER && t < t0) pm[j].look_back(mk);
+    else if (AFTER && t >= t1) run_step(cur[j], acc[j], PeriodMask::past_end(mk, cur[j] > 0), 1);
+    else run_step(cur[j], acc[j], pm[j].inside(AFTER, mk), 1);
   };
   auto open_any = [&]() { return (cur[0] | cur[1] | cur[2] | cur[3]) != 0; };
 
@@ -434,7 +408,7 @@ spell_runstat4_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t
   float res[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    acc[j].add(cur[j], cur[j] >= 1);
+    run_close(cur[j], acc[j], 1);
     res[j] = acc[j].result(reducer);
   }
   *reinterpret_cast<float4*>(out + (int64_t)p * C + c) = make_float4(res[0], res[1], res[2], res[3]);
@@ -490,7 +464,7 @@ spell_sumw_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t ldx
     for (int j = 0; j < 4; ++j) ring[k][j] = 0.0;
   int last[4] = {-1, -1, -1, -1};
   bool skip[4] = {false, false, false, false};
-  // MAX / SUM / COUNT keep a running form in acc.a; any other reducer closes runs into RunAcc<kRunAny>
+  // MAX / SUM / COUNT keep run_step's running form; any other reducer closes runs into RunAcc<kRunAny>
   constexpr bool kRunning = RED == XC_RL_MAX || RED == XC_RL_SUM || RED == XC_RL_COUNT;
   int cur[4] = {0, 0, 0, 0};
   RunAcc<kRunning ? RED : kRunAny> acc[4];
@@ -498,16 +472,8 @@ spell_sumw_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t ldx
   for (int j = 0; j < 4; ++j) acc[j].init();
   // run-length update with the mask value of the next step (cur > 0 <=> a run is open)
   auto update = [&](int j, bool mk) {
-    if constexpr (RED == XC_RL_MAX) {
-      cur[j] = mk ? cur[j] + 1 : 0;
-      acc[j].a = max(acc[j].a, cur[j]);
-    } else if constexpr (RED == XC_RL_SUM) {
-      cur[j] = mk ? 1 : 0;
-      acc[j].a += cur[j];
-    } else if constexpr (RED == XC_RL_COUNT) {
-      const int now = mk ? 1 : 0;
-      acc[j].a += now & (cur[j] ^ 1);
-      cur[j] = now;
+    if constexpr (kRunning) {
+      run_step<true>(cur[j], acc[j], mk, 1);
     } else if (mk) {
       ++cur[j];
     } else {
@@ -515,6 +481,9 @@ spell_sumw_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t ldx
       cur[j] = 0;
     }
   };
+  // The period-edge rule of runstat.cuh (PeriodMask), kept as a copy: with PeriodMask's look_back / inside / past_end
+  // in place of the lambdas below, ptxas spills 64 bytes in the W = 5 MAX, SUM and COUNT instances with
+  // resample_before_rl=False.
   // inside the period: with resample_before_rl=False a run that was already open at t0 is skipped
   auto feed_inside = [&](int j, bool mk) {
     if (AFTER) {
@@ -968,20 +937,14 @@ extern "C" int32_t xc_spell_runstat_f32(const float* x, int64_t T, int64_t C, in
   if (can_stream4(x, C, ldx, out, window)) {
     const size_t smem = (size_t)window * kThreads * 16;
     dim3 grid4((unsigned)((C / 4 + kThreads - 1) / kThreads), (unsigned)P, 1);
-    if (resample_before_rl) {
-      if (smem > 48 * 1024)
-        XC_CHECK_CUDA(cudaFuncSetAttribute(spell_runstat4_kernel<false>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      spell_runstat4_kernel<false><<<grid4, kThreads, smem, (cudaStream_t)stream>>>(
-          x, T, C, ldx, period_offsets, window, window_stat, op, (float)thr, reducer, out);
-    } else {
-      if (smem > 48 * 1024)
-        XC_CHECK_CUDA(cudaFuncSetAttribute(spell_runstat4_kernel<true>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      spell_runstat4_kernel<true><<<grid4, kThreads, smem, (cudaStream_t)stream>>>(
-          x, T, C, ldx, period_offsets, window, window_stat, op, (float)thr, reducer, out);
-    }
-    return launch_status("spell_runstat4_kernel");
+    auto go = [&](auto AFTC) -> int32_t {
+      auto kernel = spell_runstat4_kernel<decltype(AFTC)::value>;
+      if (int32_t e = allow_smem(kernel, smem, "cudaFuncSetAttribute(spell_runstat4_kernel)")) return e;
+      kernel<<<grid4, kThreads, smem, (cudaStream_t)stream>>>(x, T, C, ldx, period_offsets, window, window_stat, op,
+                                                              (float)thr, reducer, out);
+      return launch_status("spell_runstat4_kernel");
+    };
+    return resample_before_rl ? go(std::false_type{}) : go(std::true_type{});
   }
   dim3 grid((unsigned)((C + kThreads - 1) / kThreads), (unsigned)P, 1);
   spell_runstat_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(x, T, C, ldx, period_offsets, window,

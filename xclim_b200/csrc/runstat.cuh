@@ -1,17 +1,83 @@
-// Run-length reducers and per-period statistics shared by the streaming kernels: one copy of the rules.
+// Run-length reducers, period edges of the runs and per-period statistics shared by the streaming kernels: one
+// copy of the rules.  The run-length code is __host__ __device__ so that a host build can test it.
 #pragma once
 #include "common.cuh"
 
+#define XC_RS_HD __host__ __device__ __forceinline__
+
 namespace xc {
 
+// ---- row streaming: VEC adjacent cells per thread, UNROLL rows in flight ------------------------------------------
+template <int VEC>
+struct Vec;
+template <>
+struct Vec<1> {
+  float v[1];
+  __device__ __forceinline__ void load(const float* p) { v[0] = ld_stream(p); }
+};
+template <>
+struct Vec<2> {
+  float v[2];
+  __device__ __forceinline__ void load(const float* p) {
+    float2 q;
+    asm volatile("ld.global.nc.L1::no_allocate.v2.f32 {%0,%1}, [%2];" : "=f"(q.x), "=f"(q.y) : "l"(p));
+    v[0] = q.x; v[1] = q.y;
+  }
+};
+template <>
+struct Vec<4> {
+  float v[4];
+  __device__ __forceinline__ void load(const float* p) {
+    float4 q = ld_stream4(p);
+    v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
+  }
+};
+
+template <int VEC, typename T>
+__device__ __forceinline__ void store_vec(T* dst, const T (&v)[VEC]) {
+  if constexpr (VEC == 4 && sizeof(T) == 4) {
+    uint4 q;
+    q.x = *reinterpret_cast<const uint32_t*>(&v[0]);
+    q.y = *reinterpret_cast<const uint32_t*>(&v[1]);
+    q.z = *reinterpret_cast<const uint32_t*>(&v[2]);
+    q.w = *reinterpret_cast<const uint32_t*>(&v[3]);
+    *reinterpret_cast<uint4*>(dst) = q;
+  } else {
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) dst[i] = v[i];
+  }
+}
+
+// Iterate f(Vec) over the rows t in [t0, t1) with UNROLL loads in flight.
+template <int VEC, int UNROLL = 8, typename F>
+__device__ __forceinline__ void stream_rows(const float* __restrict__ col, int64_t ldx, int t0, int t1, F&& f) {
+  int t = t0;
+  const float* p = col + (int64_t)t0 * ldx;
+  for (; t + UNROLL <= t1; t += UNROLL) {
+    Vec<VEC> r[UNROLL];
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) r[u].load(p + (int64_t)u * ldx);
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) f(r[u]);
+    p += (int64_t)UNROLL * ldx;
+  }
+  for (; t < t1; ++t) {
+    Vec<VEC> r;
+    r.load(p);
+    f(r);
+    p += ldx;
+  }
+}
+
+// ---- run lengths ----------------------------------------------------------------------------------------------------
 // Reducer value of a RunAcc that keeps every quantity and picks the reducer at run time (result(int)).
 constexpr int kRunAny = -1;
 
 // mean and std of n run lengths with sum s and sum of squares q; 0 when there is no run
-__device__ __forceinline__ float run_mean(int32_t n, int32_t s) {
+XC_RS_HD float run_mean(int32_t n, int32_t s) {
   return n == 0 ? 0.f : (float)((double)s / (double)n);
 }
-__device__ __forceinline__ float run_std(int32_t n, int32_t s, unsigned long long q) {
+XC_RS_HD float run_std(int32_t n, int32_t s, unsigned long long q) {
   if (n == 0) return 0.f;
   double nn = (double)n, m = (double)s / nn;
   double var = (double)q / nn - m * m;
@@ -25,7 +91,7 @@ struct RunAcc {
   int32_t s;        // MEAN/STD/any: sum L
   unsigned long long q;  // STD/any: sum L^2
   int32_t mx, mn;   // any: max L, min L
-  __device__ __forceinline__ void init() {
+  XC_RS_HD void init() {
     a = (RED == XC_RL_MIN) ? 0x7fffffff : 0;
     s = 0;
     q = 0ull;
@@ -34,7 +100,7 @@ struct RunAcc {
       mn = 0x7fffffff;
     }
   }
-  __device__ __forceinline__ void add(int32_t L, bool take) {
+  XC_RS_HD void add(int32_t L, bool take) {
     if constexpr (RED == XC_RL_MAX) a = take ? max(a, L) : a;
     if constexpr (RED == XC_RL_MIN) a = take ? min(a, L) : a;
     if constexpr (RED == XC_RL_SUM) a += take ? L : 0;
@@ -55,7 +121,7 @@ struct RunAcc {
       }
     }
   }
-  __device__ __forceinline__ float result() const {
+  XC_RS_HD float result() const {
     if constexpr (RED == XC_RL_MAX || RED == XC_RL_SUM || RED == XC_RL_COUNT) return (float)a;
     if constexpr (RED == XC_RL_MIN) return a == 0x7fffffff ? 0.f : (float)a;
     if constexpr (RED == XC_RL_MEAN) return run_mean(a, s);
@@ -63,7 +129,7 @@ struct RunAcc {
     return 0.f;
   }
   // the reducer chosen at run time (any); a fixed RED ignores `reducer`
-  __device__ __forceinline__ float result(int reducer) const {
+  XC_RS_HD float result(int reducer) const {
     if constexpr (RED != kRunAny) return result();
     switch (reducer) {
       case XC_RL_MAX: return (float)mx;
@@ -74,6 +140,57 @@ struct RunAcc {
       default: return run_std(a, s, q);
     }
   }
+};
+
+// Run lengths of the mask a period sees into a RunAcc.  `cur` is the length of the open run (0: none; with the
+// running SUM and COUNT forms 1 while a run is open).  run_step() extends the open run with mask value m or closes it,
+// taken when it is at least `window` steps long; run_close() takes the run open at the period or series end.
+// RUNNING selects the window-1 running forms, which need no run end: MAX the largest running length, SUM the number of
+// mask steps, COUNT the number of run starts.
+template <bool RUNNING = false, int RED>
+XC_RS_HD void run_step(int32_t& cur, RunAcc<RED>& acc, bool m, int32_t window) {
+  static_assert(!RUNNING || RED == XC_RL_MAX || RED == XC_RL_SUM || RED == XC_RL_COUNT, "no running form");
+  if constexpr (RUNNING && RED == XC_RL_MAX) {
+    cur = m ? cur + 1 : 0;
+    acc.a = max(acc.a, cur);
+  } else if constexpr (RUNNING && RED == XC_RL_SUM) {
+    cur = m ? 1 : 0;
+    acc.a += cur;
+  } else if constexpr (RUNNING && RED == XC_RL_COUNT) {
+    const int32_t now = m ? 1 : 0;
+    acc.a += now & (cur ^ 1);
+    cur = now;
+  } else {
+    const int32_t L = cur;
+    acc.add(L, !m && L >= window);
+    cur = m ? L + 1 : 0;
+  }
+}
+template <bool RUNNING = false, int RED>
+XC_RS_HD void run_close(int32_t cur, RunAcc<RED>& acc, int32_t window) {
+  if constexpr (!RUNNING) acc.add(cur, cur >= window);
+}
+
+// The steps of a condition mask that make the runs of the period [t0, t1) (indices/run_length.py:87-132,
+// resample_and_rl).  Without `after` (resample_before_rl=True) they are the runs of m[t0:t1], cut at the period
+// edges.  With `after` (resample_before_rl=False) a run belongs to the period holding its FIRST step
+// (run_length.py:329-334): a run already open at t0 belongs to an earlier period and is skipped, and a run still
+// open at t1 keeps its full length past t1, where no new run may start (it would belong to a later period).
+// A kernel passes the mask at t0 - 1 to look_back() (with `after`, when t0 > 0), every step of [t0, t1) through
+// inside(), and with `after` the steps from t1 on through past_end() until its runs have closed.
+struct PeriodMask {
+  bool skip;   // the run open at t0 - 1 goes on
+  XC_RS_HD void init() { skip = false; }
+  XC_RS_HD void look_back(bool m) { skip = m; }
+  XC_RS_HD bool inside(bool after, bool m) {
+    if (after) {
+      skip = skip && m;
+      m = m && !skip;
+    }
+    return m;
+  }
+  // `open`: a run of this cell is open at the step before
+  XC_RS_HD static bool past_end(bool m, bool open) { return m && open; }
 };
 
 // Statistic of n non-NaN values with float64 sum s and sum of squares q and their min or max m.  Mean, min and
