@@ -307,6 +307,50 @@ def main():
                {"rows": Cd // X, "rolling_ms": ms_roll, "fit_ms": ms_fit, "apply_ms": ms_app,
                 "apply_elements_per_s": T * Cd / (ms_app * 1e-3), **card})
         del rd, pd_, nzd, nnd
+    if want("evfit") and a.only:    # frequency analysis: opt-in (--only evfit), on its own full-grid maxima
+        import subprocess
+        from oracle import evfit_oracle as FO
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True)
+        card = {"gpu": torch.cuda.get_device_name(), "power_limit": q.stdout.strip() or "unknown"}
+        grid, band = 721 * X, 90 * X
+        t_ret = np.array([2, 10, 20, 50, 100], np.float64)
+        for P in (30, 150):
+            # YS maxima of synthetic daily pr, made band by band (P years of daily data do not fit in HBM whole)
+            poff_y = np.arange(P + 1, dtype=np.int32) * YEAR
+            mx = torch.empty((P, grid), dtype=torch.float32, device="cuda")
+            for c0 in range(0, grid, band):
+                cb = min(band, grid - c0)
+                d = device.synth(P * YEAR, cb, kind=0, seed=5, cell_offset=c0, cells_per_lat=X, n_lat_global=721)
+                mx[:, c0:c0 + cb] = device.period_reduce(d, poff_y, _lib.STATS["max"])[0]
+                del d
+            for dist in ("genextreme", "gumbel_r"):
+                code = _lib.EV_DISTS[dist]
+                prm, status = device.ev_fit(mx, code)
+                ms_fit = timeit(lambda: device.ev_fit(mx, code), a.steps)
+                ms_tr = timeit(lambda: device.ev_transform(prm, code, _lib.EV_KINDS["isf"], 1.0 / t_ret), a.steps)
+                rl = device.ev_transform(prm, code, _lib.EV_KINDS["isf"], 1.0 / t_ret)
+                cols = np.unique(np.r_[np.linspace(0, grid - 1, 16).astype(int), np.arange(grid - 8, grid)])
+                xs, ps, rls = mx[:, cols].cpu().numpy(), prm[:, cols].cpu().numpy(), rl[:, cols].cpu().numpy()
+                worst_nnlf, worst_rl = 0.0, 0.0
+                for k in range(cols.size):
+                    po = FO.fit(xs[:, k], dist)
+                    if dist == "genextreme":
+                        fo = FO.gev_nnlf(po, xs[:, k])
+                        worst_nnlf = max(worst_nnlf, (FO.gev_nnlf(ps[:, k], xs[:, k]) - fo) / max(1.0, abs(fo)))
+                    ro = FO.return_levels(po[:, None], dist, t_ret)[:, 0]
+                    worst_rl = max(worst_rl, float(np.max(np.abs(rls[:, k] - ro) / np.abs(ro))))
+                nan_cells = int(torch.isnan(prm[0]).sum().item())
+                report(f"evfit {dist} ML fit on YS maxima, P={P} x 721 x 1440 (+ isf at T=2..100)", ms_fit,
+                       P * grid * 4 * 2 + prm.numel() * 8,
+                       {"years": P, "fit_ms": ms_fit, "fit_cells_per_s": grid / (ms_fit * 1e-3),
+                        "transform_ms": ms_tr, "transform_elements_per_s": t_ret.size * grid / (ms_tr * 1e-3),
+                        "bound": "FP64 pipe: log1p / exp of every value in every Newton iteration",
+                        "status": status, "nan_cells": nan_cells,
+                        "oracle_check": {"cells": int(cols.size), "max_rel_nnlf_excess": worst_nnlf,
+                                         "max_return_level_rel_diff": worst_rl}, **card})
+                del prm, rl
+            del mx
     if want("fwi") and a.only:      # the fire-weather kernel: opt-in (--only fwi), never part of a default run
         import time
 

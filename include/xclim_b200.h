@@ -620,6 +620,43 @@ int32_t xc_si_apply_f32(const float* x, int64_t T, int64_t C, int64_t ldx, const
                         int64_t ldo, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * s2  Frequency analysis -- indices/stats.py
+ *   Replaces the per-cell scipy fit of `fit` (:115-218: `_fitfunc_1d` :45-112 with `_fit_start` :576-610,
+ *   method ML, then scipy's norm_gen.fit / gumbel_r_gen.fit / rv_continuous.fit) and the per-cell scipy ppf /
+ *   isf / cdf of `parametric_quantile` (:221-289) and `parametric_cdf` (:294-360), which `fa` (:429-475) and
+ *   `frequency_analysis` (:478-548) call.
+ * ------------------------------------------------------------------------------------------- */
+#define XC_EV_NORM       0   /* params (loc, scale) */
+#define XC_EV_GUMBEL_R   1   /* params (loc, scale) */
+#define XC_EV_GENEXTREME 2   /* params (c, loc, scale), scipy's sign of c */
+#define XC_EV_PPF 0
+#define XC_EV_ISF 1
+#define XC_EV_CDF 2
+/* status word bits, OR-ed over all cells */
+#define XC_EV_STATUS_NOT_CONVERGED 1   /* the Newton iterations did not converge (the cell is NaN) */
+#define XC_EV_STATUS_UNBOUNDED     2   /* no maximum of the likelihood (NaN): genextreme ran into c -> 1, or
+                                          gumbel_r / genextreme on a sample of one repeated value */
+#define XC_EV_STATUS_ROOT_NAN      4   /* gumbel_r: the scale equation is NaN at a bracket end (scipy raises) */
+#define XC_EV_STATUS_ROOT_SIGN     8   /* gumbel_r: no sign change on [0, inf] (scipy raises) */
+
+/* Bytes of the fit workspace: one float32 per cell and step. */
+int64_t xc_ev_fit_workspace_bytes(int64_t T, int64_t C);
+/* Fit `dist` by maximum likelihood to the finite values of each column x[t * ldx + c], t < T (device float32;
+ * NaN and +-inf dropped as np.ma.masked_invalid does).  params (device float64, (2 | 3, C)): scipy's order,
+ * NaN for a column with <= 1 finite value or any NaN parameter.  norm is scipy's closed form bit for bit,
+ * gumbel_r the root of scipy's scale equation to a few ulp, genextreme the optimum of the likelihood (Newton in
+ * (c, loc, log scale) from xclim's start).  *status (device int32, OR-ed, caller zeroes it) gets
+ * XC_EV_STATUS_* bits. */
+int32_t xc_ev_fit_f32(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t dist, double* params,
+                      int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
+/* out[j * C + c] (device float64, (nq, C)) = scipy's `dist.ppf(q[j], *p)`, `dist.isf(q[j], *p)` or
+ * `dist.cdf(q[j], *p)` (kind XC_EV_*) with p the column c of params ((2 | 3, C) device float64); q device
+ * float64 (nq <= 65535).  rv_continuous's argument checks: NaN for scale <= 0, a non-finite shape, a NaN loc or
+ * a probability outside [0, 1]. */
+int32_t xc_ev_transform_f64(const double* params, int64_t C, int32_t dist, int32_t kind, const double* q,
+                            int32_t nq, double* out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * e1  Ensemble statistics across realizations -- ensembles/_base.py, ensembles/_robustness.py
  *   The ensemble is an (R, N) matrix of N independent columns, x[r * ldr + n] (device float32, ldr >= N: a lat
  *   tile of a wider buffer is a column range with the buffer's member stride).  1 <= R <= XC_ENS_MAX_MEMBERS.

@@ -83,6 +83,9 @@ SIGNATURES = {
                              _vp, _i64, _vp]),
     "xc_si_apply_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _f64, _f64, _f64, _vp,
                                _i64, _vp]),
+    "xc_ev_fit_workspace_bytes": (_i64, [_i64, _i64]),
+    "xc_ev_fit_f32": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _i64, _vp]),
+    "xc_ev_transform_f64": (_i32, [_vp, _i64, _i32, _i32, _vp, _i32, _vp, _vp]),
     "xc_ens_percentiles_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _f64, _f64, _i32, _vp, _vp]),
     "xc_ens_moments_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "xc_ens_robustness_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64,
@@ -98,6 +101,11 @@ ENS_FRACTIONS = ("changed", "positive", "changed_positive", "negative", "changed
 SI_DISTS = {"gamma": 0, "fisk": 1, "lognorm": 2}
 SI_METHODS = {"APP": 0, "ML": 1}
 SI_STATUS_FITDATA, SI_STATUS_ROOT_NAN, SI_STATUS_ROOT_SIGN, SI_STATUS_LOGNORM_FALLBACK = 1, 2, 4, 8
+
+# frequency analysis (include/xclim_b200.h s2)
+EV_DISTS = {"norm": 0, "gumbel_r": 1, "genextreme": 2}
+EV_KINDS = {"ppf": 0, "isf": 1, "cdf": 2}
+EV_STATUS_NOT_CONVERGED, EV_STATUS_UNBOUNDED, EV_STATUS_ROOT_NAN, EV_STATUS_ROOT_SIGN = 1, 2, 4, 8
 
 
 

@@ -609,6 +609,36 @@ def si_apply(x2d, group_of_step, params, n_zeros, n_notnull, dist_code, interp=1
     return out
 
 
+# ------------------------------------------------------------------------------------ frequency analysis
+def ev_fit(x2d, dist_code):
+    """Fit every column of the (T, C) float32 series (xc_ev_fit_f32).  Returns ``(params (2 | 3, C) float64,
+    status int)``; reading the status synchronises the stream."""
+    T, C = x2d.shape
+    lib = load()
+    ws = torch.empty(int(lib.xc_ev_fit_workspace_bytes(T, C)), dtype=torch.uint8, device=x2d.device)
+    params = torch.empty((3 if dist_code == _lib.EV_DISTS["genextreme"] else 2, C), dtype=torch.float64,
+                         device=x2d.device)
+    status = torch.zeros(1, dtype=torch.int32, device=x2d.device)
+    check(lib.xc_ev_fit_f32(x2d.data_ptr(), T, C, x2d.stride(0), int(dist_code), params.data_ptr(),
+                            status.data_ptr(), ws.data_ptr(), ws.numel(), current_stream_ptr()))
+    return params, int(status.item())
+
+
+def ev_transform(params, dist_code, kind_code, q):
+    """(nq, C) float64 ppf / isf / cdf of the fitted laws (xc_ev_transform_f64); ``params`` (2 | 3, C) float64
+    tensor (copied to the device when it is not there), ``q`` host probabilities or values."""
+    P, C = params.shape
+    if not params.is_cuda:
+        _require_cuda()
+        params = params.to("cuda")
+    params = params.to(torch.float64).contiguous()
+    qd = torch.as_tensor(np.ascontiguousarray(q, dtype=np.float64).ravel()).to(params.device)
+    out = torch.empty((qd.numel(), C), dtype=torch.float64, device=params.device)
+    check(load().xc_ev_transform_f64(params.data_ptr(), C, int(dist_code), int(kind_code), qd.data_ptr(),
+                                     qd.numel(), out.data_ptr(), current_stream_ptr()))
+    return out
+
+
 # ------------------------------------------------------------------------------------ ensembles
 def ens_percentiles(x2d, percentiles, alpha, beta, min_members):
     """Percentiles along the member axis of an (R, N) float32 matrix (xc_ens_percentiles_f32; column views with

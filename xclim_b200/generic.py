@@ -158,6 +158,32 @@ def select_resample_op(da, op, freq="YS", out_units=None, **indexer):
     return _wrap_periods(da, out, cell_shape, other, ta, freq, attrs, dtype=dtype)
 
 
+_MONTH_ABBREVIATIONS = {1: "JAN", 2: "FEB", 3: "MAR", 4: "APR", 5: "MAY", 6: "JUN", 7: "JUL", 8: "AUG", 9: "SEP",
+                        10: "OCT", 11: "NOV", 12: "DEC"}
+
+
+def default_freq(**indexer):
+    """Default resampling frequency of an indexer -- indices/generic.py:224-252: "YS-JAN", or the year starting
+    in the indexer's first month ("YS-DEC" for a season)."""
+    freq = "YS-JAN"
+    if indexer:
+        group, value = indexer.popitem()
+        if group == "season":
+            month = 12      # the "season" scheme is based on YS-DEC
+        elif group == "month":
+            month = int(np.take(value, 0))
+        elif group == "doy_bounds":
+            # the month of day value[0] of 2004 (a leap year), as cftime.num2date(value[0] - 1, "days since
+            # 2004-01-01") gives it
+            month = int((np.datetime64("2004-01-01") + np.timedelta64(int(value[0]) - 1, "D")).astype(object).month)
+        elif group == "date_bounds":
+            month = int(value[0][:2])
+        else:
+            raise ValueError(f"Unknown group `{group}`.")
+        freq = "YS-" + _MONTH_ABBREVIATIONS[month]
+    return freq
+
+
 def cumulative_difference(data, threshold, op, freq=None):
     """Sum of the excess over (deficit under) a threshold -- indices/generic.py:1514-1552."""
     code = get_op(op, constrain=(">", ">=", "<", "<="))

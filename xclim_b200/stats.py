@@ -295,3 +295,218 @@ def standardized_index(da, freq, window, dist, method, zero_inflated, fitkwargs,
     if not is_xarray(da) and series.gdim == "dayofyear":
         time = time_axis_of(da)
     return wrap_like(da, vals, ("time",) + tuple(other), time=time, attrs=attrs)
+
+
+# ------------------------------------------------------------------------ frequency analysis (stats.py:115-548)
+_FIT_METHOD_NAMES = {"ML": "maximum likelihood", "MM": "method of moments", "MLE": "maximum likelihood",
+                     "MSE": "maximum product of spacings", "MPS": "maximum product of spacings",
+                     "PWM": "probability weighted moments", "APP": "approximative method"}
+_EV_PARAM_NAMES = {"norm": ["loc", "scale"], "gumbel_r": ["loc", "scale"], "genextreme": ["c", "loc", "scale"]}
+
+
+def _ev_dist(dist):
+    """get_dist (stats.py:551-573) for the laws the frequency-analysis kernels cover."""
+    if not isinstance(dist, str):
+        raise NotImplementedError("rv_continuous distribution objects are not supported by the xclim_b200 hot path")
+    if dist in _EV_PARAM_NAMES:
+        return dist
+    try:
+        import scipy.stats
+        known = getattr(scipy.stats, dist, None) is not None
+    except ImportError:     # pragma: no cover - scipy only tells an unknown name from an unsupported one
+        known = True
+    if not known:
+        raise ValueError(f"Statistical distribution `{dist}` is not found in scipy.stats.")
+    raise NotImplementedError(f"The distribution `{dist}` is not supported by the xclim_b200 frequency analysis "
+                              f"(supported: {', '.join(_EV_PARAM_NAMES)}).")
+
+
+def _prefix_attrs(attrs, names, prefix):
+    return {(prefix + k if k in names else k): v for k, v in attrs.items()}
+
+
+def _unprefix_attrs(attrs, names, prefix):
+    """xclim.core.formatting.unprefix_attrs: a prefixed key wins over the plain one."""
+    out = {}
+    for k, v in attrs.items():
+        if k.startswith(prefix) and k[len(prefix):] in names:
+            out[k[len(prefix):]] = v
+        elif k not in out:
+            out[k] = v
+    return out
+
+
+def _history(text, name):
+    from datetime import datetime
+    return f"[{datetime.now().strftime('%Y-%m-%d %H:%M:%S')}] {name}: {text} - xclim_b200"
+
+
+def _output(template, out_dev, lead_dims_shape, dims, coords, attrs):
+    vals = out_dev.reshape(lead_dims_shape)
+    vals = vals if (OPTIONS["device_outputs"] and not is_xarray(template)) else vals.cpu().numpy()
+    return wrap_like(template, vals, dims, coords_extra=coords, attrs=attrs)
+
+
+def fit(da, dist="norm", method="ML", dim="time", **fitkwargs):
+    """Fit a univariate law along time, per cell -- indices/stats.py:115-218.  float64, ``dparams`` in place of
+    ``time``, coordinates in scipy's order.  Maximum likelihood (``ML`` / ``MLE``) of ``norm``, ``gumbel_r`` and
+    ``genextreme`` (xc_ev_fit_f32); NaN and +-inf values are dropped, a cell with <= 1 value left is NaN."""
+    method = method.upper()
+    if method not in _FIT_METHOD_NAMES:
+        raise ValueError(f"Fitting method not recognized: {method}")
+    dist = _ev_dist(dist)
+    if method == "PWM":
+        raise ValueError(f"The given distribution {dist} does not implement the PWM fitting method. "
+                         "Please pass an instance from the lmoments3 package.")
+    if method not in ("ML", "MLE"):
+        why = {"MM": "scipy runs its generic moment-matching optimiser there",
+               "APP": "the approximative method has no start values for these laws",
+               "MSE": "scipy.stats.fit's spacing optimiser is not reproduced",
+               "MPS": "scipy.stats.fit's spacing optimiser is not reproduced"}[method]
+        raise NotImplementedError(f"method {method!r} is not supported by the xclim_b200 frequency analysis: {why}")
+    if dim != "time":
+        raise NotImplementedError(f"fits along {dim!r} are not supported: the kernels fit along `time`")
+    if fitkwargs:
+        raise NotImplementedError(f"fitkwargs {sorted(fitkwargs)} (fixed parameters, optimiser options) are not "
+                                  "supported by the xclim_b200 frequency analysis")
+    dims = dims_of(da)
+    if "time" not in dims:
+        raise ValueError("input must have a `time` dimension")
+    x2d, cell_shape = device.to_time_cell(raw_values(da), dims.index("time"))
+    params, status = device.ev_fit(x2d, _lib.EV_DISTS[dist])
+    if status & _lib.EV_STATUS_ROOT_NAN:
+        raise ValueError("The function value at a bracket end is NaN; solver cannot continue.")
+    if status & _lib.EV_STATUS_ROOT_SIGN:
+        raise ValueError("f(a) and f(b) must have different signs")
+    if status & (_lib.EV_STATUS_NOT_CONVERGED | _lib.EV_STATUS_UNBOUNDED):
+        import torch
+        fitted = torch.isfinite(x2d).sum(0) > 1
+        bad = int((fitted & torch.isnan(params[0])).sum().item())
+        why = "the likelihood has no maximum (c >= 1) or the Newton iterations did not converge"
+        warnings.warn(f"{dist} fit: {bad} cell(s) set to NaN: {why}", RuntimeWarning)
+    names = _EV_PARAM_NAMES[dist]
+    ti = dims.index("time")
+    out = params.reshape((len(names),) + tuple(cell_shape))
+    out = out.permute(*([k for k in range(1, ti + 1)] + [0] + [k for k in range(ti + 1, len(dims))]))
+    out_dims = tuple(d if d != "time" else "dparams" for d in dims)
+    attrs = _prefix_attrs(attrs_of(da), ["standard_name", "long_name", "units", "description"], "original_")
+    attrs.update({"long_name": f"{dist} parameters", "description": f"Parameters of the {dist} distribution",
+                  "method": method, "estimator": _FIT_METHOD_NAMES[method].capitalize(), "scipy_dist": dist,
+                  "units": "",
+                  "history": _history(f"Estimate distribution parameters by {_FIT_METHOD_NAMES[method]} method "
+                                      f"along dimension {dim}.", "fit")})
+    return _output(da, out.contiguous(), tuple(out.shape), out_dims, {"dparams": names}, attrs)
+
+
+def _params_2d(p, dist):
+    """A fitted-parameters array -> ((P, C) float64 tensor, its dims, dparams position, cell shape)."""
+    import torch
+    dims = dims_of(p)
+    if "dparams" not in dims:
+        raise ValueError("the parameters need a `dparams` dimension")
+    vals = raw_values(p)
+    t = vals if isinstance(vals, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(vals, np.float64))
+    t = t.to(torch.float64)
+    k = dims.index("dparams")
+    if t.shape[k] != len(_EV_PARAM_NAMES[dist]):
+        raise ValueError(f"{dist} has {len(_EV_PARAM_NAMES[dist])} parameters, `dparams` has {t.shape[k]}")
+    t = t.movedim(k, 0).contiguous()
+    rest = tuple(t.shape[1:])
+    return t.reshape(t.shape[0], -1), dims, k, rest
+
+
+def _transformed(p, dist, kind, q, new_dim, coord, attrs):
+    params, dims, k, rest = _params_2d(p, dist)
+    if params.shape[1] == 0:
+        import torch
+        out = torch.empty((len(q), 0), dtype=torch.float64, device=params.device)
+    else:
+        out = device.ev_transform(params, _lib.EV_DISTS[dist], _lib.EV_KINDS[kind], q)
+    out = out.reshape((len(q),) + rest).movedim(0, k).contiguous()
+    out_dims = tuple(d if d != "dparams" else new_dim for d in dims)
+    return _output(p, out, tuple(out.shape), out_dims, {new_dim: coord}, attrs)
+
+
+def _quantiles(p, q, dist, new_dim, coord):
+    dist = _ev_dist(dist or attrs_of(p)["scipy_dist"])
+    attrs = _unprefix_attrs(attrs_of(p), ["units", "standard_name"], "original_")
+    attrs.update({"long_name": f"{dist} quantiles", "description": f"Quantiles estimated by the {dist} distribution",
+                  "cell_methods": "dparams: ppf",
+                  "history": _history("Compute parametric quantiles from distribution parameters",
+                                      "parametric_quantile")})
+    if np.all(q > 0.5):
+        return _transformed(p, dist, "isf", 1 - q, new_dim, coord, attrs)
+    return _transformed(p, dist, "ppf", q, new_dim, coord, attrs)
+
+
+def parametric_quantile(p, q, dist=None):
+    """Quantiles of the fitted laws -- indices/stats.py:221-289: ``isf(1 - q)`` when every q > 0.5, else
+    ``ppf(q)``; ``dparams`` becomes ``quantile`` (xc_ev_transform_f64)."""
+    q = np.atleast_1d(q)
+    return _quantiles(p, q, dist, "quantile", q)
+
+
+def parametric_cdf(p, v, dist=None):
+    """CDF of the fitted laws at the values ``v`` -- indices/stats.py:294-360; ``dparams`` becomes ``cdf``."""
+    if hasattr(v, "dims"):
+        if len(v.dims) > 1:
+            raise ValueError("`v` must be one-dimensional.")
+        v = np.asarray(v.values)
+    v = np.atleast_1d(v)
+    dist = _ev_dist(dist or attrs_of(p)["scipy_dist"])
+    attrs = _unprefix_attrs(attrs_of(p), ["units", "standard_name"], "original_")
+    attrs.update({"long_name": f"{dist} cdf", "description": f"CDF estimated by the {dist} distribution",
+                  "cell_methods": "dparams: cdf",
+                  "history": _history("Compute parametric cdf from distribution parameters", "parametric_cdf")})
+    return _transformed(p, dist, "cdf", np.asarray(v, np.float64), "cdf", v, attrs)
+
+
+def fa(da, t, dist="norm", mode="max", method="ML"):
+    """Return levels -- indices/stats.py:429-475: the value of return period ``t`` (exceedance for ``mode``
+    max / high, non-exceedance for min / low); output dim ``return_period``."""
+    p = fit(da, dist, method=method)
+    t = np.atleast_1d(t)
+    if mode in ["max", "high"]:
+        q = 1 - 1.0 / t
+    elif mode in ["min", "low"]:
+        q = 1.0 / t
+    else:
+        raise ValueError(f"Mode `{mode}` should be either 'max' or 'min'.")
+    out = _quantiles(p, q, dist, "return_period", t)
+    out.attrs["mode"] = mode
+    return out
+
+
+def _extremes(da, mode, window, freq, **indexer):
+    """The per-period extremes of frequency_analysis (stats.py:526-538): rolling mean (skipna=False), then
+    select_resample_op(op=mode) with the indexer."""
+    from . import generic
+    from .units import to_agg_units_attrs
+    dims = dims_of(da)
+    if "time" not in dims:
+        raise ValueError("input must have a `time` dimension")
+    x2d, cell_shape = device.to_time_cell(raw_values(da), dims.index("time"))
+    other = tuple(d for d in dims if d != "time")
+    ta = time_axis_of(da)
+    if int(window) > 1:
+        x2d = device.rolling_mean(x2d, int(window))
+    if indexer:
+        keep = ta.select_mask(**indexer)
+        if not keep.all():
+            x2d = device.mask_steps(x2d, keep)
+    out, _ = device.period_reduce(x2d, ta.period_offsets(freq), _lib.STATS[mode])
+    attrs = attrs_of(da)
+    attrs.update(to_agg_units_attrs(da, mode))
+    return generic._wrap_periods(da, out, tuple(cell_shape), other, ta, freq, attrs)
+
+
+def frequency_analysis(da, mode, t, dist, window=1, freq=None, method="ML", **indexer):
+    """Return levels of the per-period extremes -- indices/stats.py:478-548.  Host-backed inputs stream through
+    HBM in slabs for the extremes (xclim_b200/streaming.py); only the (periods, cells) extremes are fitted."""
+    from . import generic
+    from .streaming import streamed
+    if mode not in ("max", "min"):
+        raise ValueError(f"Mode `{mode}` should be either 'max' or 'min'.")
+    freq = freq or generic.default_freq(**indexer)
+    sel = streamed(_extremes)(da, mode, window, freq, **indexer)
+    return fa(sel, t, dist=dist, mode=mode, method=method)
