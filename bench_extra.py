@@ -351,6 +351,47 @@ def main():
                                          "max_return_level_rel_diff": worst_rl}, **card})
                 del prm, rl
             del mx
+    if want("analog") and a.only:   # spatial analogues: opt-in (--only analog), one target against the full grid
+        import subprocess
+        from oracle import analog_oracle as AO
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True)
+        card = {"gpu": torch.cuda.get_device_name(), "power_limit": q.stdout.strip() or "unknown"}
+        grid, n, m, d = 721 * X, 30, 30, 3
+        g = torch.Generator(device="cuda").manual_seed(17)
+        shift = torch.randn((1, d, grid), generator=g, device="cuda")
+        cand = (torch.randn((m, d, grid), generator=g, device="cuda") + shift).contiguous()
+        tgt = cand[:, :, 1234].contiguous()[None].clone()                   # (1, n, d): one cell's own sample
+        tx = tgt[0].double().cpu().numpy()
+        cols = np.unique(np.r_[np.linspace(0, grid - 33, 224).astype(int), np.arange(grid - 32, grid)])
+        ys = cand[:, :, cols].double().cpu().numpy()
+        N, pairs = n + m, (n + m) * (n + m - 1) // 2
+        # algorithmic float64 operations per cell (a sqrt or log counts as one): the pair loops dominate
+        flops = {"seuclidean": 4 * N * d, "mahalanobis": 4 * N * d + 2 * d * d,
+                 "zech_aslan": pairs * (4 * d + 2), "szekely_rizzo": pairs * (4 * d + 2),
+                 "nearest_neighbor": N * (N - 1) * 3 * d, "kldiv": n * N * 3 * d + 2 * n,
+                 "kolmogorov_smirnov": 0}
+        for method, param in (("seuclidean", 0.0), ("nearest_neighbor", 0.0), ("zech_aslan", 1e-12),
+                              ("szekely_rizzo", 1.0), ("kolmogorov_smirnov", 0.0), ("kldiv", 1.0),
+                              ("mahalanobis", 0.0)):
+            cst = AO.target_consts(tx, method)
+            cst = None if cst is None else torch.from_numpy(np.asarray(cst).reshape(1, -1)).cuda()
+            code = _lib.AN_METHODS[method]
+            out, status = device.analog(tgt, cand, code, param, cst)
+            ms = timeit(lambda: device.analog(tgt, cand, code, param, cst), a.steps)
+            got = out[0, cols].cpu().numpy()
+            kw = {"zech_aslan": {"dmin": param}, "kldiv": {"k": 1}}.get(method, {})
+            ref = np.array([AO.metric(method, tx, ys[:, :, k], **kw) for k in range(cols.size)])
+            worst = float(np.max(np.abs(got - ref) / np.maximum(np.abs(ref), 1e-300)))
+            fl = flops[method] * grid
+            extra = {"method": method, "cells": grid, "n": n, "m": m, "d": d, "status": status,
+                     "fp64_ops": fl, "fp64_ops_per_s": fl / (ms * 1e-3),
+                     "share_of_fp64_peak": fl / (ms * 1e-3) / 34e12,
+                     "oracle_check": {"cells": int(cols.size), "max_rel_diff": worst}, **card}
+            if method == "kolmogorov_smirnov":
+                extra["comparisons"] = 2 * n * (2 * N * d + N * N) * grid
+            report(f"analog {method}, n = m = 30, d = 3, 721 x 1440 cells", ms, cand.numel() * 4 + grid * 8, extra)
+        del cand, shift
     if want("fwi") and a.only:      # the fire-weather kernel: opt-in (--only fwi), never part of a default run
         import time
 

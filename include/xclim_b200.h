@@ -657,6 +657,35 @@ int32_t xc_ev_transform_f64(const double* params, int64_t C, int32_t dist, int32
                             int32_t nq, double* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * a1  Spatial analogues -- analog.py
+ *   Replaces the per-cell metric call of `spatial_analogs` (:87-97, xr.apply_ufunc(vectorize=True)) with
+ *   `_metric_overhead` (:154-170) and the metrics `seuclidean` (:181-213), `nearest_neighbor` (:216-251),
+ *   `zech_aslan` (:254-319), `szekely_rizzo` (:322-385), `kolmogorov_smirnov` (:433-495), `kldiv` (:498-587)
+ *   and `mahalanobis` (:590-628).  Everything is float64 from the float32 samples (DESIGN.md section 4).
+ * ------------------------------------------------------------------------------------------- */
+#define XC_AN_SEUCLIDEAN         0   /* consts (K, d): the target's var(ddof=1) */
+#define XC_AN_NEAREST_NEIGHBOR   1
+#define XC_AN_ZECH_ASLAN         2   /* param: dmin */
+#define XC_AN_SZEKELY_RIZZO      3   /* param: standardize (0 or 1) */
+#define XC_AN_KOLMOGOROV_SMIRNOV 4
+#define XC_AN_KLDIV              5   /* param: k, 1 <= k <= XC_AN_KLDIV_MAX_K; d <= 10 */
+#define XC_AN_MAHALANOBIS        6   /* consts (K, d, d): the inverse covariance VI */
+#define XC_AN_MAX_D        16
+#define XC_AN_KLDIV_MAX_K  16
+/* status word bits, OR-ed over all (target, cell) pairs: the reference raises ValueError for the whole call */
+#define XC_AN_STATUS_NOT_FINITE 1   /* nearest_neighbor / kldiv: cKDTree's "data must be finite, check for nan
+                                       or inf values" (a non-finite standardized value, or +-inf for kldiv) */
+#define XC_AN_STATUS_CHKFINITE  2   /* seuclidean: scipy.linalg.norm's "array must not contain infs or NaNs" */
+/* out[t * C + c] (device float64, (K, C)) = metric(target t, candidate cell c).  target: device float32 (K, n, d)
+ * contiguous; cand: device float32 (m, d, C) at cand[(s * d + k) * ldc + c], ldc >= C.  NaN anywhere in either
+ * sample gives NaN (:154-156).  consts: device float64 per target for seuclidean and mahalanobis (NULL
+ * otherwise).  *status (device int32, caller zeroes it) gets XC_AN_STATUS_* bits.  Returns XC_ERR_INVALID for
+ * bad shapes, an unknown method or a sample too large for one CTA's shared memory. */
+int32_t xc_analog_f32(const float* target, int64_t n, int64_t K, const float* cand, int64_t m, int64_t C,
+                      int64_t ldc, int64_t d, int32_t method, double param, const double* consts, double* out,
+                      int32_t* status, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * e1  Ensemble statistics across realizations -- ensembles/_base.py, ensembles/_robustness.py
  *   The ensemble is an (R, N) matrix of N independent columns, x[r * ldr + n] (device float32, ldr >= N: a lat
  *   tile of a wider buffer is a column range with the buffer's member stride).  1 <= R <= XC_ENS_MAX_MEMBERS.

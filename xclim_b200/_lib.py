@@ -86,6 +86,7 @@ SIGNATURES = {
     "xc_ev_fit_workspace_bytes": (_i64, [_i64, _i64]),
     "xc_ev_fit_f32": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _i64, _vp]),
     "xc_ev_transform_f64": (_i32, [_vp, _i64, _i32, _i32, _vp, _i32, _vp, _vp]),
+    "xc_analog_f32": (_i32, [_vp, _i64, _i64, _vp, _i64, _i64, _i64, _i64, _i32, _f64, _vp, _vp, _vp, _vp]),
     "xc_ens_percentiles_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _f64, _f64, _i32, _vp, _vp]),
     "xc_ens_moments_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "xc_ens_robustness_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64,
@@ -107,7 +108,11 @@ EV_DISTS = {"norm": 0, "gumbel_r": 1, "genextreme": 2}
 EV_KINDS = {"ppf": 0, "isf": 1, "cdf": 2}
 EV_STATUS_NOT_CONVERGED, EV_STATUS_UNBOUNDED, EV_STATUS_ROOT_NAN, EV_STATUS_ROOT_SIGN = 1, 2, 4, 8
 
-
+# spatial analogues (include/xclim_b200.h a1)
+AN_METHODS = {"seuclidean": 0, "nearest_neighbor": 1, "zech_aslan": 2, "szekely_rizzo": 3, "kolmogorov_smirnov": 4,
+              "kldiv": 5, "mahalanobis": 6}
+AN_MAX_D, AN_KLDIV_MAX_K = 16, 16
+AN_STATUS_NOT_FINITE, AN_STATUS_CHKFINITE = 1, 2
 
 # ---- plan of the fused multi-output pass (include/xclim_b200.h: XcMultiPlan)
 MULTI_MAX_COND, MULTI_MAX_RUNS, MULTI_MAX_MSUM, MULTI_MAX_SUMS = 6, 4, 1, 3

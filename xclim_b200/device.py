@@ -639,6 +639,22 @@ def ev_transform(params, dist_code, kind_code, q):
     return out
 
 
+# ------------------------------------------------------------------------------------ spatial analogues
+def analog(target, cand, method_code, param, consts):
+    """(K, C) float64 dissimilarities (xc_analog_f32) of the (K, n, d) float32 targets against the (m, d, C) float32
+    candidates (unit cell stride; a row stride > C works in place), with ``consts`` the (K, d | d * d) float64
+    per-target constants or None.  Returns ``(out, status)``; reading the status synchronises the stream."""
+    K, n, d = target.shape
+    m, _, C = cand.shape
+    assert target.dtype == torch.float32 and target.is_contiguous()
+    assert cand.dtype == torch.float32 and cand.stride(2) == 1 and cand.stride(0) == d * cand.stride(1)
+    out = torch.empty((K, C), dtype=torch.float64, device=cand.device)
+    status = torch.zeros(1, dtype=torch.int32, device=cand.device)
+    check(load().xc_analog_f32(target.data_ptr(), n, K, cand.data_ptr(), m, C, cand.stride(1), d, int(method_code),
+                               float(param), _ptr(consts), out.data_ptr(), status.data_ptr(), current_stream_ptr()))
+    return out, int(status.item())
+
+
 # ------------------------------------------------------------------------------------ ensembles
 def ens_percentiles(x2d, percentiles, alpha, beta, min_members):
     """Percentiles along the member axis of an (R, N) float32 matrix (xc_ens_percentiles_f32; column views with
