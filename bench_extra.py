@@ -392,6 +392,83 @@ def main():
                 extra["comparisons"] = 2 * n * (2 * N * d + N * N) * grid
             report(f"analog {method}, n = m = 30, d = 3, 721 x 1440 cells", ms, cand.numel() * 4 + grid * 8, extra)
         del cand, shift
+    if want("pet") and a.only:      # evapotranspiration: opt-in (--only pet), on the --lat band of the grid
+        import subprocess
+        from oracle import pet_oracle as PO
+        from xclim_b200 import TimeAxis, converters
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True)
+        card = {"gpu": torch.cuda.get_device_name(), "power_limit": q.stdout.strip() or "unknown"}
+        ta = TimeAxis.daily("1981-01-01", T, "noleap")
+        lat_u = np.linspace(-89.5, 89.5, a.lat)
+        idx = np.repeat(np.arange(a.lat, dtype=np.int32), X)
+        idx_d = torch.from_numpy(idx).cuda()
+        cols = np.unique(np.r_[np.linspace(0, C - 1, 96).astype(int), np.arange(C - 32, C)])
+
+        def params(method, wb, affine):
+            P = _lib.PetParams()
+            P.method, P.water_budget = _lib.PET_METHODS[method], int(wb)
+            for i, name in enumerate(_lib.PET_INPUTS):
+                P.in_scale[i], P.in_offset[i] = affine.get(name, (1.0, 0.0))
+            P.wind_num, P.wind_den = float(np.log(67.8 * 2 - 5.42)), float(np.log(67.8 * 10 - 5.42))
+            return P
+
+        def ins(**kw):
+            return [kw.get(n) for n in _lib.PET_INPUTS]
+
+        def sample(x):
+            return x[:, cols].cpu().numpy()
+
+        tmin = tas - 5.0
+        tmax = tas + 5.0
+        degf = {"tasmin": (1.8, -459.67), "tasmax": (1.8, -459.67)}
+        table = torch.from_numpy(converters._daily_table("BR65", ta, lat_u)).cuda()
+        P = params("BR65", True, degf)
+        out = device.pet_daily(ins(tasmin=tmin, tasmax=tmax, pr=pr), table, idx_d, P)
+        ms = timeit(lambda: device.pet_daily(ins(tasmin=tmin, tasmax=tmax, pr=pr), table, idx_d, P), a.steps)
+        f = lambda x: (x * np.float32(1.8) + np.float32(-459.67)).astype(np.float32)   # noqa: E731
+        ref = np.float32(PO.daily_rate(PO.daily_pet("BR65", table.cpu().numpy()[:, idx[cols]], tasmin=f(sample(tmin)),
+                                                    tasmax=f(sample(tmax))), sample(pr)))
+        got = sample(out)
+        report(f"pet BR65 water budget, {a.lat} x 1440 cells", ms, 4 * (3 + 1) * T * C,
+               {"oracle_check": {"cells": int(cols.size), "bit_equal": bool(np.array_equal(got, ref, equal_nan=True))},
+                **card})
+        del out, table
+        # FAO_PM98 on a 40-row band: eight input series
+        C8 = 40 * X
+        g = torch.Generator(device="cuda").manual_seed(5)
+        ser = {k: (torch.rand((T, C8), generator=g, device="cuda") * s + o)
+               for k, s, o in (("tasmin", 10, 270), ("tasmax", 10, 280), ("hurs", 0.9, 0.1), ("rsds", 300, 0),
+                               ("rsus", 60, 0), ("rlds", 200, 200), ("rlus", 250, 200), ("sfcWind", 10, 0))}
+        k2c = {"tasmin": (1.0, -273.15), "tasmax": (1.0, -273.15)}
+        P = params("allen98", False, k2c)
+        out = device.pet_daily(ins(**ser), None, None, P)
+        ms = timeit(lambda: device.pet_daily(ins(**ser), None, None, P), a.steps)
+        c8 = np.unique(np.r_[np.linspace(0, C8 - 1, 96).astype(int), np.arange(C8 - 32, C8)])
+        sm = {k: v[:, c8].cpu().numpy() for k, v in ser.items()}
+        for k in ("tasmin", "tasmax"):
+            sm[k] = (sm[k] * np.float32(1.0) + np.float32(-273.15)).astype(np.float32)
+        ref = np.float32(PO.daily_rate(PO.daily_pet("allen98", None, **sm)))
+        got = out[:, c8].cpu().numpy()
+        ulp = float(np.max(np.abs(got.view(np.int32).astype(np.int64) - ref.view(np.int32).astype(np.int64))))
+        report("pet FAO_PM98, 40 x 1440 cells", ms, 4 * (8 + 1) * T * C8,
+               {"cells": C8, "oracle_check": {"cells": int(c8.size), "max_ulp": ulp}, **card})
+        del ser, out
+        # TW48 from the daily tas, monthly output
+        moff, yoff, ym, mdays = converters._months(ta)
+        mtab = torch.from_numpy(converters._monthly_table("TW48", ta, ym, lat_u)).cuda()
+        P = params("TW48", False, {"tas": (1.0, -273.15)})
+        out = device.pet_monthly(ins(tas=tas), moff, yoff, mdays, mtab, idx_d, P)
+        ms = timeit(lambda: device.pet_monthly(ins(tas=tas), moff, yoff, mdays, mtab, idx_d, P), a.steps)
+        tsm = (sample(tas) * np.float32(1.0) + np.float32(-273.15)).astype(np.float32)
+        ref = np.float32(PO.monthly_pet("TW48", ta.year, ta.month, ta.doy, "noleap", lat_u[idx[cols]], tas=tsm))
+        got = out[:, cols].cpu().numpy()
+        fin = np.isfinite(ref)
+        ulp = float(np.max(np.abs(got[fin].view(np.int32).astype(np.int64) - ref[fin].view(np.int32).astype(np.int64))))
+        report(f"pet TW48, {a.lat} x 1440 cells", ms, 4 * T * C + 4 * len(ym) * C,
+               {"oracle_check": {"cells": int(cols.size), "max_ulp": ulp,
+                                 "nan_match": bool(np.array_equal(np.isnan(got), np.isnan(ref)))}, **card})
+        del out, tmin, tmax
     if want("fwi") and a.only:      # the fire-weather kernel: opt-in (--only fwi), never part of a default run
         import time
 

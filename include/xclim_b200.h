@@ -732,6 +732,62 @@ int32_t xc_ens_robustness_f32(const float* fut, int64_t Tf, int64_t ldf_r, int64
                               const double* weights, int32_t test, double param, int32_t strict_sign,
                               double* fractions, float* pvals, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * p1  Potential evapotranspiration and the water budget -- indices/converters.py
+ *   Replaces `potential_evapotranspiration` (:1890-2152) and `water_budget` (:2652-2739) on daily inputs.
+ *   The solar terms (extraterrestrial radiation, day length: indices/helpers.py:95-525) depend on (day,
+ *   latitude) only; the host tabulates them once per (row, distinct latitude) in float64 and the kernels read
+ *   table[row * L + lat_index[c]].  Each input is loaded as float32, mapped by its affine unit conversion
+ *   (x * in_scale + in_offset, in float32) and the formula is evaluated in float64, rounded once to float32.
+ *   Output unit: kg m-2 s-1 (the reference's amount2rate + hydro conversion, :2149-2151).
+ * ------------------------------------------------------------------------------------------- */
+#define XC_PET_BR65   0   /* tasmin, tasmax [degF]; table: radiation [cal cm-2 d-1]          :2000-2009 */
+#define XC_PET_HG85   1   /* tasmin, tasmax, tas (optional) [degC]; table: 0.408 * ra [MJ m-2 d-1] :2011-2027 */
+#define XC_PET_MB05   2   /* tas, or tasmin and tasmax [degC]; table: radiation (1367 W m-2) [J m-2 d-1]
+                                                                                          :2060-2080 */
+#define XC_PET_ALLEN98 3  /* tasmin, tasmax [degC], hurs [1], rsds, rsus, rlds, rlus [W m-2], sfcWind [m s-1];
+                             no table                                                       :2116-2144 */
+#define XC_PET_TW48   4   /* monthly: tas, or tasmin and tasmax [degC]; table: mean day length / 12 :2082-2114 */
+#define XC_PET_DA02   5   /* monthly: tasmin, tasmax, tas (optional) [degC], pr [mm/month]; table: 0.408 * the
+                             monthly sum of ra [MJ m-2 d-1]                                 :2029-2058 */
+#define XC_PET_GIVEN  6   /* daily water budget from a given evspsblpot [kg m-2 s-1]; no table  :2732-2733 */
+/* input slots of XcPetParams / the inputs array */
+#define XC_PET_IN_TASMIN 0
+#define XC_PET_IN_TASMAX 1
+#define XC_PET_IN_TAS    2
+#define XC_PET_IN_HURS   3
+#define XC_PET_IN_RSDS   4
+#define XC_PET_IN_RSUS   5
+#define XC_PET_IN_RLDS   6
+#define XC_PET_IN_RLUS   7
+#define XC_PET_IN_WIND   8
+#define XC_PET_IN_PR     9   /* the precipitation of DA02 [mm/month], or of the fused water budget [kg m-2 s-1] */
+#define XC_PET_IN_EVSPSBLPOT 10
+#define XC_PET_N_IN     11
+typedef struct {
+  int32_t method;          /* XC_PET_* */
+  int32_t water_budget;    /* 1: out = pr - pet (pr in slot XC_PET_IN_PR, kg m-2 s-1), 0: out = pet */
+  float in_scale[XC_PET_N_IN], in_offset[XC_PET_N_IN];
+  double peta, petb;       /* MB05 coefficients (:1903-1904) */
+  double wind_num, wind_den;  /* allen98: sfcWind at 2 m = sfcWind * wind_num / wind_den, the log law of
+                                 helpers.py:809-849 from 10 m (log(67.8 * 2 - 5.42), log(67.8 * 10 - 5.42)) */
+} XcPetParams;
+/* Daily methods (BR65, HG85, MB05, allen98, GIVEN).  inputs: host array of XC_PET_N_IN device float32 pointers,
+ * NULL where unused, each (T, C) at x[t * ldx + c], ldx >= C.  table: device float64 (T, L); lat_index: device
+ * int32 (C) in [0, L) (allen98, GIVEN: both may be NULL).  out: device float32 (T, C) at out[t * ldx + c]. */
+int32_t xc_pet_daily_f32(const float* const* inputs, int64_t T, int64_t C, int64_t ldx, const double* table,
+                         int64_t L, const int32_t* lat_index, const XcPetParams* params_host, float* out,
+                         void* stream);
+/* Monthly methods (TW48, DA02) from daily inputs.  moff: device int32 (M + 1) row offsets of the M calendar
+ * months the series touches; yoff: device int32 (Y + 1) month offsets of the years (YS groups) those months
+ * fall in (TW48's annual heat index; a group of more than 12 months gives NaN months); mdays: device float64 (M) days of each complete month.  table: device
+ * float64 (M, L).  Monthly means are skipna (an all-NaN month is NaN).  out: device float32 (M, C),
+ * out[m * C + c].  The fused water budget (TW48 only) subtracts from pr's monthly mean. */
+int32_t xc_pet_monthly_f32(const float* const* inputs, int64_t T, int64_t C, int64_t ldx, const int32_t* moff,
+                           int64_t M, const int32_t* yoff, int64_t Y, const double* mdays, const double* table,
+                           int64_t L, const int32_t* lat_index, const XcPetParams* params_host, float* out,
+                           void* stream);
+
 #ifdef __cplusplus
 }
 #endif

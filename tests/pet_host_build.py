@@ -1,0 +1,83 @@
+"""TEST INFRASTRUCTURE: build and bind the host build of the evapotranspiration device code
+(tests/csrc/pet_host.cpp over xclim_b200/csrc/pet_core.cuh), behind the argument lists of device.pet_daily and
+device.pet_monthly with numpy arrays in place of device tensors."""
+import ctypes
+import os
+import subprocess
+import tempfile
+
+import numpy as np
+
+from xclim_b200 import _lib as L
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+ROOT = os.path.dirname(HERE)
+_lib = None
+_vp, _i64, _i32 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32
+
+
+def load():
+    global _lib
+    if _lib is None:
+        out = os.path.join(tempfile.gettempdir(), f"libxclim_b200_pet_host_{os.getuid()}.so")
+        src = os.path.join(HERE, "csrc", "pet_host.cpp")
+        deps = [src, os.path.join(ROOT, "include", "xclim_b200.h"), os.path.join(ROOT, "xclim_b200", "csrc", "pet_core.cuh")]
+        if not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
+            tmp = out + f".{os.getpid()}.tmp"
+            cmd = ["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", src, "-o", tmp]
+            subprocess.run(cmd, check=True, capture_output=True, text=True)
+            os.replace(tmp, out)
+        lib = ctypes.CDLL(out)
+        lib.pet_host_daily.restype = _i32
+        lib.pet_host_daily.argtypes = [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _vp]
+        lib.pet_host_monthly.restype = _i32
+        lib.pet_host_monthly.argtypes = [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp]
+        _lib = lib
+    return _lib
+
+
+def _p(a):
+    return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
+
+
+def _inputs(inputs):
+    arrs = [None if x is None else np.ascontiguousarray(x, dtype=np.float32) for x in inputs]
+    ref = next(x for x in arrs if x is not None)
+    return arrs, (ctypes.c_void_p * len(arrs))(*[_p(x) for x in arrs]), ref.shape
+
+
+def params(method, water_budget=False, affine=None, peta=0.00516409319477, petb=0.0874972822289):
+    P = L.PetParams()
+    P.method, P.water_budget = L.PET_METHODS[method], int(water_budget)
+    for i in range(len(L.PET_INPUTS)):
+        P.in_scale[i], P.in_offset[i] = (affine or {}).get(L.PET_INPUTS[i], (1.0, 0.0))
+    P.peta, P.petb = peta, petb
+    P.wind_num, P.wind_den = float(np.log(67.8 * 2 - 5.42)), float(np.log(67.8 * 10 - 5.42))
+    return P
+
+
+def daily(inputs, table, lat_index, P):
+    """(T, C) float32 of the host build; ``inputs``: the XC_PET_N_IN (T, C) arrays or None.  Raises ValueError
+    where the C ABI rejects the arguments."""
+    keep, ptrs, (T, C) = _inputs(inputs)
+    tab = None if table is None else np.ascontiguousarray(table, dtype=np.float64)
+    li = None if lat_index is None else np.ascontiguousarray(lat_index, dtype=np.int32)
+    out = np.full((T, C), np.nan, dtype=np.float32)
+    st = load().pet_host_daily(ptrs, T, C, C, _p(tab), 0 if tab is None else tab.shape[1], _p(li),
+                               ctypes.byref(P), _p(out))
+    if st:
+        raise ValueError("invalid arguments")
+    return out
+
+
+def monthly(inputs, moff, yoff, mdays, table, lat_index, P):
+    keep, ptrs, (T, C) = _inputs(inputs)
+    moff, yoff = np.ascontiguousarray(moff, np.int32), np.ascontiguousarray(yoff, np.int32)
+    mdays, tab = np.ascontiguousarray(mdays, np.float64), np.ascontiguousarray(table, np.float64)
+    li = np.ascontiguousarray(lat_index, np.int32)
+    out = np.full((moff.size - 1, C), np.nan, dtype=np.float32)
+    st = load().pet_host_monthly(ptrs, T, C, C, _p(moff), moff.size - 1, _p(yoff), yoff.size - 1, _p(mdays), _p(tab),
+                                 tab.shape[1], _p(li), ctypes.byref(P), _p(out))
+    if st:
+        raise ValueError("invalid arguments")
+    return out

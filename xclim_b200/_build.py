@@ -33,9 +33,11 @@ NVCC_FLAGS = [
 #: dqm.cu (the trend, detrend and retrend of the oracle, operation by operation) and stdindex.cu (numpy's float32
 #: moment expressions of the distribution fit) and ensemble.cu (the float64 moments and t-tests that the CPU tests
 #: build for the host) and evfit.cu (numpy's float32 normal fit and the likelihood fits the CPU tests build for
-#: the host) and analog.cu (the dissimilarity metrics the CPU tests build for the host).
+#: the host) and analog.cu (the dissimilarity metrics the CPU tests build for the host) and pet.cu (the
+#: evapotranspiration formulas the CPU tests build for the host).
 EXTRA_FLAGS = {"fwi.cu": ["-fmad=false"], "dqm.cu": ["-fmad=false"], "stdindex.cu": ["-fmad=false"],
-               "ensemble.cu": ["-fmad=false"], "evfit.cu": ["-fmad=false"], "analog.cu": ["-fmad=false"]}
+               "ensemble.cu": ["-fmad=false"], "evfit.cu": ["-fmad=false"], "analog.cu": ["-fmad=false"],
+               "pet.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:

@@ -87,6 +87,8 @@ SIGNATURES = {
     "xc_ev_fit_f32": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _i64, _vp]),
     "xc_ev_transform_f64": (_i32, [_vp, _i64, _i32, _i32, _vp, _i32, _vp, _vp]),
     "xc_analog_f32": (_i32, [_vp, _i64, _i64, _vp, _i64, _i64, _i64, _i64, _i32, _f64, _vp, _vp, _vp, _vp]),
+    "xc_pet_daily_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "xc_pet_monthly_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "xc_ens_percentiles_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _f64, _f64, _i32, _vp, _vp]),
     "xc_ens_moments_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "xc_ens_robustness_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64,
@@ -113,6 +115,18 @@ AN_METHODS = {"seuclidean": 0, "nearest_neighbor": 1, "zech_aslan": 2, "szekely_
               "kldiv": 5, "mahalanobis": 6}
 AN_MAX_D, AN_KLDIV_MAX_K = 16, 16
 AN_STATUS_NOT_FINITE, AN_STATUS_CHKFINITE = 1, 2
+
+# potential evapotranspiration (include/xclim_b200.h p1)
+PET_METHODS = {"BR65": 0, "HG85": 1, "MB05": 2, "allen98": 3, "TW48": 4, "DA02": 5, "given": 6}
+PET_MONTHLY = ("TW48", "DA02")
+PET_INPUTS = ("tasmin", "tasmax", "tas", "hurs", "rsds", "rsus", "rlds", "rlus", "sfcWind", "pr", "evspsblpot")
+
+
+class PetParams(C.Structure):
+    """include/xclim_b200.h XcPetParams."""
+    _fields_ = [("method", _i32), ("water_budget", _i32), ("in_scale", C.c_float * 11), ("in_offset", C.c_float * 11),
+                ("peta", _f64), ("petb", _f64), ("wind_num", _f64), ("wind_den", _f64)]
+
 
 # ---- plan of the fused multi-output pass (include/xclim_b200.h: XcMultiPlan)
 MULTI_MAX_COND, MULTI_MAX_RUNS, MULTI_MAX_MSUM, MULTI_MAX_SUMS = 6, 4, 1, 3

@@ -655,6 +655,50 @@ def analog(target, cand, method_code, param, consts):
     return out, int(status.item())
 
 
+# ------------------------------------------------------------------------------------ evapotranspiration
+def _pet_inputs(inputs):
+    """Host array of the XC_PET_N_IN input pointers and (T, C, ld) of the (T, C) float32 device series."""
+    import ctypes
+    ref = next(x for x in inputs if x is not None)
+    T, C = ref.shape
+    ld = ref.stride(0)
+    for x in inputs:
+        if x is not None and (tuple(x.shape) != (T, C) or x.stride(0) != ld or x.stride(1) != 1
+                              or x.dtype != torch.float32):
+            raise ValueError("pet: the inputs must share their (T, C) float32 layout")
+    return (ctypes.c_void_p * len(inputs))(*[_ptr(x) for x in inputs]), T, C, ld, ref.device
+
+
+def pet_daily(inputs, table, lat_index, params):
+    """PET or the water budget of a daily method (xc_pet_daily_f32): ``inputs`` the XC_PET_N_IN (T, C) float32
+    device series or None (a row stride > C works in place), ``table`` (T, L) float64 and ``lat_index`` (C,) int32
+    device tensors (None for allen98), ``params`` a ``_lib.PetParams``.  Returns (T, C) float32 with the row stride
+    of the inputs."""
+    import ctypes
+    ptrs, T, C, ld, dev = _pet_inputs(inputs)
+    out = torch.empty((T, ld), dtype=torch.float32, device=dev)[:, :C]
+    L = 0 if table is None else table.shape[1]
+    check(load().xc_pet_daily_f32(ptrs, T, C, ld, _ptr(table), L, _ptr(lat_index), ctypes.byref(params),
+                                  out.data_ptr(), current_stream_ptr()))
+    return out
+
+
+def pet_monthly(inputs, moff, yoff, mdays, table, lat_index, params):
+    """PET or the water budget of a monthly method (xc_pet_monthly_f32) from daily series: ``moff`` (M + 1) and
+    ``yoff`` (Y + 1) int32 host arrays, ``mdays`` (M,) float64 host array, ``table`` (M, L) float64 and
+    ``lat_index`` (C,) int32 device tensors.  Returns (M, C) float32."""
+    import ctypes
+    ptrs, T, C, ld, dev = _pet_inputs(inputs)
+    moff_d, yoff_d = dev_ints(moff, np.int32, dev), dev_ints(yoff, np.int32, dev)
+    mdays_d = torch.from_numpy(np.ascontiguousarray(mdays, dtype=np.float64)).to(dev)
+    M = moff_d.numel() - 1
+    out = torch.empty((M, C), dtype=torch.float32, device=dev)
+    check(load().xc_pet_monthly_f32(ptrs, T, C, ld, moff_d.data_ptr(), M, yoff_d.data_ptr(), yoff_d.numel() - 1,
+                                    mdays_d.data_ptr(), table.data_ptr(), table.shape[1], lat_index.data_ptr(),
+                                    ctypes.byref(params), out.data_ptr(), current_stream_ptr()))
+    return out
+
+
 # ------------------------------------------------------------------------------------ ensembles
 def ens_percentiles(x2d, percentiles, alpha, beta, min_members):
     """Percentiles along the member axis of an (R, N) float32 matrix (xc_ens_percentiles_f32; column views with

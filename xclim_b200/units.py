@@ -22,7 +22,12 @@ _ALIASES = {
     "mm": "mm", "d": "d", "days": "d", "day": "d", "": "", "1": "", "m/s": "m s-1", "m s-1": "m s-1",
     "km h-1": "km h-1", "km/h": "km h-1", "kph": "km h-1", "km hr-1": "km h-1",
     "kg/m**2/s": "kg m-2 s-1", "kg m**-2 s**-1": "kg m-2 s-1",
+    "%": "%", "percent": "%", "pct": "%",
+    "w m-2": "W m-2", "w/m2": "W m-2", "w m^-2": "W m-2", "w m**-2": "W m-2", "w/m^2": "W m-2", "w/m**2": "W m-2",
+    "mm/month": "mm/month", "mm month-1": "mm/month",
 }
+#: pint's default registry: month = year / 12, year = 365.25 d
+_DAYS_PER_MONTH = 365.25 / 12
 
 
 def _canon(u: str) -> str:
@@ -52,6 +57,14 @@ def _to_base(v: float, u: str):
         return v / 86400.0, "prflux"
     if u == "kg m-2 s-1":
         return v, "prflux"
+    if u == "mm/month":
+        return v / (86400.0 * _DAYS_PER_MONTH), "prflux"
+    if u == "%":
+        return v / 100.0, "ratio"
+    if u == "":
+        return v, "ratio"
+    if u == "W m-2":
+        return v, "radflux"
     if u == "m s-1":
         return v, "speed"
     if u == "km h-1":
@@ -70,6 +83,10 @@ def _from_base(v: float, u: str):
         return v * 86400.0
     if u == "km h-1":
         return v * 3.6
+    if u == "mm/month":
+        return v * (86400.0 * _DAYS_PER_MONTH)
+    if u == "%":
+        return v * 100.0
     return v
 
 
