@@ -469,6 +469,94 @@ def main():
                {"oracle_check": {"cells": int(cols.size), "max_ulp": ulp,
                                  "nan_match": bool(np.array_equal(np.isnan(got), np.isnan(ref)))}, **card})
         del out, tmin, tmax
+    if want("etccdi") and a.only:   # day-of-year percentile indices: opt-in (--only etccdi)
+        import subprocess
+        from oracle import etccdi_oracle as EO
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True)
+        card = {"gpu": torch.cuda.get_device_name(), "power_limit": q.stdout.strip() or "unknown",
+                "frac_basis": "3.35 TB/s (H100 SXM data sheet)"}
+        gt, gw = _lib.OPS[">"], _lib.RL_REDUCERS["sum"]
+
+        def frac(nbytes, ms):
+            return nbytes / (ms * 1e-3) / 3.35e12
+
+        def rel(got, exp):
+            got, exp = np.asarray(got, np.float64), np.asarray(exp, np.float64)
+            with np.errstate(invalid="ignore", divide="ignore"):
+                d = np.abs(got - exp) / np.maximum(np.abs(exp), 1e-30)
+            return float(np.nanmax(np.where(np.isnan(got) & np.isnan(exp), 0.0, d)))
+
+        # WSDI and tx90p on the full (10950, 721, 1440) grid, one lat tile at a time (30-year tx90 table per tile)
+        del tas, pr
+        torch.cuda.empty_cache()
+        rows = 120
+        tot = {"wsdi": 0.0, "tx90p": 0.0}
+        nbytes = {"wsdi": 0, "tx90p": 0}
+        worst, checked = 0, 0
+        for r0 in range(0, 721, rows):
+            nr = min(rows, 721 - r0)
+            Ct = nr * X
+            x = device.synth(T, Ct, kind=1, seed=3, cell_offset=r0 * X, cells_per_lat=X, n_lat_global=721)
+            tab = device.percentile_doy(x, doy, yidx, YEAR, T // YEAR, 5, [90.0], 1 / 3, 1 / 3)[0]
+            out, _ = device.doy_runstat(x, poff, doy, tab, gt, gw, 6, True)
+            tot["wsdi"] += timeit(lambda: device.doy_runstat(x, poff, doy, tab, gt, gw, 6, True), a.steps)
+            tot["tx90p"] += timeit(lambda: device.doy_threshold_count(x, poff, doy, tab, gt), a.steps)
+            for k in tot:
+                nbytes[k] += 4 * T * Ct + 8 * YEAR * Ct + 4 * (len(poff) - 1) * Ct
+            if r0 == 0 or r0 + rows >= 721:          # sampled cells of the first and the last tile
+                cols = np.unique(np.r_[np.linspace(0, Ct - 1, 64).astype(int), np.arange(Ct - 16, Ct)])
+                exp = EO.warm_spell_duration_index(x[:, cols].cpu().numpy(), tab[:, cols].cpu().numpy(), doy, poff)
+                worst = max(worst, int(np.sum(out[:, cols].cpu().numpy() != exp)))
+                checked += cols.size
+            del x, tab, out
+            torch.cuda.empty_cache()
+        for k, name in (("wsdi", "warm_spell_duration_index window 6"), ("tx90p", "tx90p count")):
+            report(f"{name}, 721 x 1440 cells (lat tiles of {rows})", tot[k], nbytes[k],
+                   {"grid": [T, 721, X], "cells_per_s": 721 * X / (tot[k] * 1e-3), "frac_of_3_35_tbs": frac(nbytes[k], tot[k]),
+                    "wsdi_over_tx90p": tot["wsdi"] / tot["tx90p"],
+                    "oracle_check": {"cells": checked, "mismatches": worst}, **card})
+        # the band of --lat rows: fraction_over_precip_thresh, one compound index, DTR
+        tas = device.synth(T, C, kind=1, seed=3, cells_per_lat=X, n_lat_global=a.lat)
+        pr = device.synth(T, C, kind=0, seed=2, cells_per_lat=X, n_lat_global=a.lat)
+        cols = np.unique(np.r_[np.linspace(0, C - 1, 96).astype(int), np.arange(C - 32, C)])
+        ptab = torch.clamp(device.percentile_doy(pr, doy, yidx, YEAR, T // YEAR, 5, [95.0], 1 / 3, 1 / 3)[0], min=1.0)
+        s_thr, s_wet = device.period_sums_thr(pr, poff, gt, ptab, 1.0, doy_index=doy)
+        ms = timeit(lambda: device.period_sums_thr(pr, poff, gt, ptab, 1.0, doy_index=doy), a.steps)
+        got = (s_thr / s_wet)[:, cols].cpu().numpy()
+        exp = EO.fraction_over_precip_thresh(pr[:, cols].cpu().numpy(), ptab[:, cols].cpu().numpy(), 1.0, poff, doy=doy)
+        nb = 4 * T * C + 8 * YEAR * C + 8 * (len(poff) - 1) * C
+        report(f"fraction_over_precip_thresh (R95pTOT), {a.lat} x 1440 cells", ms, nb,
+               {"frac_of_3_35_tbs": frac(nb, ms), "oracle_check": {"cells": int(cols.size), "max_rel_diff": rel(got, exp)},
+                **card})
+        del s_thr, s_wet
+        ttab = device.percentile_doy(tas, doy, yidx, YEAR, T // YEAR, 5, [75.0], 1 / 3, 1 / 3)[0]
+        ptab75 = device.percentile_doy(pr, doy, yidx, YEAR, T // YEAR, 5, [75.0], 1 / 3, 1 / 3)[0]
+        lt = _lib.OPS["<"]
+        out = device.doy_count2(tas, pr, poff, doy, ttab, ptab75, lt, gt)
+        ms = timeit(lambda: device.doy_count2(tas, pr, poff, doy, ttab, ptab75, lt, gt), a.steps)
+        exp = EO.compound_days("cold_and_wet_days", tas[:, cols].cpu().numpy(), pr[:, cols].cpu().numpy(),
+                               ttab[:, cols].cpu().numpy(), ptab75[:, cols].cpu().numpy(), doy, poff)
+        nb = 8 * T * C + 16 * YEAR * C + 4 * (len(poff) - 1) * C
+        report(f"cold_and_wet_days, {a.lat} x 1440 cells", ms, nb,
+               {"frac_of_3_35_tbs": frac(nb, ms),
+                "oracle_check": {"cells": int(cols.size),
+                                 "mismatches": int(np.sum(out[:, cols].cpu().numpy() != exp))}, **card})
+        del ttab, ptab75, ptab, out
+        torch.cuda.empty_cache()
+        tmax = tas + torch.rand_like(tas) * 12
+        for variability in (False, True):
+            out = device.period_range_stat(tas, tmax, poff, _lib.STATS["mean"], variability)
+            ms = timeit(lambda: device.period_range_stat(tas, tmax, poff, _lib.STATS["mean"], variability), a.steps)
+            lo_s, hi_s = tas[:, cols].cpu().numpy(), tmax[:, cols].cpu().numpy()
+            exp = EO.daily_temperature_range_variability(lo_s, hi_s, poff) if variability else \
+                EO.daily_temperature_range(lo_s, hi_s, poff)
+            nb = 8 * T * C + 4 * (len(poff) - 1) * C
+            report(f"daily_temperature_range{'_variability' if variability else ''}, {a.lat} x 1440 cells", ms, nb,
+                   {"frac_of_3_35_tbs": frac(nb, ms),
+                    "oracle_check": {"cells": int(cols.size), "max_rel_diff": rel(out[:, cols].cpu().numpy(), exp)},
+                    **card})
+        del tmax, out
     if want("fwi") and a.only:      # the fire-weather kernel: opt-in (--only fwi), never part of a default run
         import time
 

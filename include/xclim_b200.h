@@ -316,6 +316,47 @@ int32_t xc_doy_threshold_count_years_f32(const float* x, int64_t T, int64_t C, i
                                          int32_t* out_count, int32_t* valid_count, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * d1  the remaining ETCCDI day-of-year percentile indices.  Every comparison against a table is in
+ *   float64 (the reference's `resample_doy` array), the threshold of step t being
+ *   table[(doy_index[t] - 1) * C + c] as for xc_doy_threshold_count_f32.
+ * ------------------------------------------------------------------------------------------- */
+/* Run statistic of `x op table[doy]` per period, as xc_period_runstat_f32 (reducer, window,
+ * resample_before_rl, valid_count): warm_spell_duration_index / cold_spell_duration_index
+ * (indices/_multivariate.py:69-153, 1719-1795: rl.windowed_run_count == XC_RL_SUM).  op is one of
+ * > < >= <=. */
+int32_t xc_doy_runstat_f32(const float* x, int64_t T, int64_t C, int64_t ldx,
+                           const int32_t* period_offsets, int32_t P,
+                           const int16_t* doy_index, const double* table, int32_t n_doy,
+                           int32_t op, int32_t reducer, int32_t window, int32_t resample_before_rl,
+                           float* out, int32_t* valid_count, void* stream);
+
+/* The two sums of fraction_over_precip_thresh (indices/_multivariate.py:1238-1297) from one read of x:
+ *   out_sum_thr[p, c] = sum of x[t, c] over t in p with (double)x op thr[row(t) * thr_rstride + c],
+ *   out_sum_wet[p, c] = sum of x[t, c] over t in p with x op (float)wet,
+ * row(t) = doy_index[t] - 1, or t when doy_index is NULL (thr_rstride = 0: one threshold per cell).
+ * Sums are float64 in time order, rounded once to float32.  op is > or >=. */
+int32_t xc_period_sums_thr_f32(const float* x, int64_t T, int64_t C, int64_t ldx,
+                               const int32_t* period_offsets, int32_t P, const int16_t* doy_index,
+                               const double* thr, int64_t thr_rstride, int32_t op, double wet,
+                               float* out_sum_thr, float* out_sum_wet, void* stream);
+
+/* Days with (x1 op1 table1[doy]) AND (x2 op2 table2[doy]) per period (float32 counts): the compound
+ * percentile days cold_and_dry_days ... cold_and_wet_days (indices/_multivariate.py:162-416).
+ * x1, x2 share (T, C, ldx); both tables are (n_doy, C); op1, op2 are > < >= <=. */
+int32_t xc_doy_count2_f32(const float* x1, const float* x2, int64_t T, int64_t C, int64_t ldx,
+                          const int32_t* period_offsets, int32_t P, const int16_t* doy_index,
+                          const double* table1, const double* table2, int32_t n_doy,
+                          int32_t op1, int32_t op2, float* out, void* stream);
+
+/* Per-period statistic `stat` (XC_STAT_*, NaN skipped) of d[t] = hi[t] - lo[t] in float32:
+ * daily_temperature_range (indices/_multivariate.py:514-557).  variability != 0: the mean of
+ * |d[t] - d[t-1]| over the steps t >= 1 of the period (the first one reaches into the previous
+ * period), daily_temperature_range_variability (:561-598); stat must then be XC_STAT_MEAN. */
+int32_t xc_period_range_stat_f32(const float* lo, const float* hi, int64_t T, int64_t C, int64_t ldx,
+                                 const int32_t* period_offsets, int32_t P, int32_t stat,
+                                 int32_t variability, float* out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * a17  percentile bootstrap (Zhang 2005) -- core/bootstrapping.py:81-211, 235-282
  *   x: (T, C) studied series; the base (climatology) period is the n_base_years equal-length
  *   year blocks of year_len steps starting at row base_start (noleap / 360_day calendars,

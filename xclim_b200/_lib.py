@@ -53,6 +53,11 @@ SIGNATURES = {
     "xc_doy_interp_f64": (_i32, [_vp, _i32, _i64, _i32, _i32, _vp, _vp]),
     "xc_doy_threshold_count_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "xc_doy_threshold_count_years_f32": (_i32, [_vp, _i64, _i64, _i64, _i64, _i32, _i32, _vp, _i32, _vp, _vp, _vp]),
+    "xc_doy_runstat_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp,
+                                  _vp]),
+    "xc_period_sums_thr_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _i64, _i32, _f64, _vp, _vp, _vp]),
+    "xc_doy_count2_f32": (_i32, [_vp, _vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "xc_period_range_stat_f32": (_i32, [_vp, _vp, _i64, _i64, _i64, _vp, _i32, _i32, _i32, _vp, _vp]),
     "xc_bootstrap_doy_count_f32": (_i32, [_vp, _i64, _i64, _i64, _i64, _i32, _i32, _vp, _i32, _i32, _f64, _f64,
                                           _f64, _i32, _vp, _vp, _vp]),
     "xc_eqm_train_workspace_bytes": (_i64, [_i64, _i64, _i32]),

@@ -57,17 +57,20 @@ period_count_kernel(const float* __restrict__ x, int64_t C, int64_t ldx,
 // run-length statistics
 // ------------------------------------------------------------------------------------------------
 // FASTMAX: reducer == max and window == 1 takes run_step's running form, which needs no run-end detection
-// (this is the maximum_consecutive_dry_days configuration).
-template <int OP, int RED, int VEC, bool VALID, bool AFTER, bool FASTMAX>
+// (this is the maximum_consecutive_dry_days configuration).  THR: the threshold source (runstat.cuh), a scalar or a
+// day-of-year table (warm / cold spell duration indices, indices/_multivariate.py:69-153, 1719-1795).
+template <int OP, int RED, int VEC, bool VALID, bool AFTER, bool FASTMAX, typename THR = ScalarThr>
 __global__ void __launch_bounds__(kThreads)
 period_runstat_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t ldx,
-                      const int32_t* __restrict__ poff, float thr, int32_t window,
+                      const int32_t* __restrict__ poff, typename ThrParam<THR>::type thr_param, int32_t window,
                       float* __restrict__ out, int32_t* __restrict__ valid) {
+  using Row = typename THR::template Row<VEC>;
   const int64_t c0 = ((int64_t)blockIdx.x * kThreads + threadIdx.x) * VEC;
   if (c0 >= C) return;
   const int p = blockIdx.y;
   const int t0 = poff[p], t1 = poff[p + 1];
   const float* col = x + c0;
+  const THR thr = ThrParam<THR>::get(thr_param);
 
   int32_t cur[VEC], nv[VEC];
   PeriodMask pm[VEC];
@@ -78,16 +81,18 @@ period_runstat_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t
   if constexpr (AFTER) {
     if (t0 > 0) {
       Vec<VEC> r;
+      Row th;
       r.load(col + (int64_t)(t0 - 1) * ldx);
+      thr.load(th, c0, t0 - 1);
 #pragma unroll
-      for (int i = 0; i < VEC; ++i) pm[i].look_back(cmp<OP>(r.v[i], thr));
+      for (int i = 0; i < VEC; ++i) pm[i].look_back(cmp<OP>(r.v[i], thr.at(th, i)));
     }
   }
 
-  stream_rows<VEC>(col, ldx, t0, t1, [&](const Vec<VEC>& r) {
+  stream_rows_thr<VEC>(col, ldx, t0, t1, thr, c0, [&](const Vec<VEC>& r, const Row& th) {
 #pragma unroll
     for (int i = 0; i < VEC; ++i) {
-      const bool c = cmp<OP>(r.v[i], thr);
+      const bool c = cmp<OP>(r.v[i], thr.at(th, i));
       if constexpr (VALID) nv[i] += (r.v[i] == r.v[i]) ? 1 : 0;
       run_step<FASTMAX>(cur[i], acc[i], pm[i].inside(AFTER, c), window);
     }
@@ -100,11 +105,13 @@ period_runstat_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t
     for (int i = 0; i < VEC; ++i) open = open || (cur[i] > 0);
     for (int t = t1; open && t < (int)T; ++t) {
       Vec<VEC> r;
+      Row th;
       r.load(col + (int64_t)t * ldx);
+      thr.load(th, c0, t);
       open = false;
 #pragma unroll
       for (int i = 0; i < VEC; ++i) {
-        const bool c = PeriodMask::past_end(cmp<OP>(r.v[i], thr), cur[i] > 0);
+        const bool c = PeriodMask::past_end(cmp<OP>(r.v[i], thr.at(th, i)), cur[i] > 0);
         run_step<FASTMAX>(cur[i], acc[i], c, window);
         open = open || c;
       }
@@ -281,41 +288,40 @@ int32_t check_common(const void* x, int64_t T, int64_t C, int64_t ldx, const voi
 
 
 // ------------------------------------------------------------------------------------------------
-// threshold count against a float64 threshold that varies by cell: a day-of-year table (indices/_multivariate.py:
-// 1583-1590, `tx90p` & family, with `resample_doy` as an index into the table) or an array (indices/generic.py:
-// 301-361 with a DataArray threshold).  numpy compares float32 data with a float64 threshold in float64 (SURVEY.md
-// A.1); each threshold is folded to the float32 one with the same truth table (fold_f64), so that the element test
-// is one float32 compare.
+// threshold count against a float64 threshold that varies by cell (TableThr, runstat.cuh): a day-of-year table
+// (indices/_multivariate.py:1583-1590, `tx90p` & family, with `resample_doy` as an index into the table) or an array
+// (indices/generic.py:301-361 with a DataArray threshold).
 //   out[p, c] = #{ t in p : x[t, c] op thr[row(t) * rstride + c] },  row(t) = doy[t] - 1, or t without doy
 // (rstride = 0: one threshold per cell).  The grid is (period, cell block) with the period fastest, so that the
 // blocks of one cell range run together and share the threshold rows through L2.  U steps of data and thresholds
 // are in flight before any use.
+// SUMS (fraction_over_precip_thresh, indices/_multivariate.py:1283-1295) sums instead of counting, from the same
+// read of x:  out[p, c] = sum of the x[t, c] that pass the table test,  valid[p, c] = sum of the x[t, c] with
+// x op wet (the float32 wet-day threshold).  Both add float32 values into a float64 sum in time order and round it
+// to float32 once, as period_reduce_kernel's conditional sum (thresholded_statistics, reducer "sum") does.
 // ------------------------------------------------------------------------------------------------
-template <int VEC>
-__device__ __forceinline__ void load_thr(const double* p, double (&t)[VEC]) {
-  if constexpr (VEC == 4) {
-    const double2 a = *reinterpret_cast<const double2*>(p), b = *reinterpret_cast<const double2*>(p + 2);
-    t[0] = a.x; t[1] = a.y; t[2] = b.x; t[3] = b.y;
-  } else {
-    t[0] = *p;
-  }
-}
-
-template <int OP, int VEC, bool VALID, bool DOY>
+template <int OP, int VEC, bool VALID, bool DOY, bool SUMS = false>
 __global__ void __launch_bounds__(kThreads)
 period_count_thr_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, const int32_t* __restrict__ poff,
                         const int16_t* __restrict__ doy, const double* __restrict__ thr, int64_t rstride,
-                        int32_t* __restrict__ out, int32_t* __restrict__ valid) {
+                        std::conditional_t<SUMS, float, int32_t>* __restrict__ out,
+                        std::conditional_t<SUMS, float, int32_t>* __restrict__ valid, float wet) {
   constexpr int U = 4;
   const int p = blockIdx.x;
   const int64_t c0 = ((int64_t)blockIdx.y * kThreads + threadIdx.x) * VEC;
   if (c0 >= C) return;
   const int t0 = poff[p], t1 = poff[p + 1];
   int32_t cnt[VEC], nv[VEC];
+  double s_thr[VEC], s_wet[VEC];
 #pragma unroll
   for (int i = 0; i < VEC; ++i) { cnt[i] = 0; nv[i] = 0; }
+  if constexpr (SUMS) {
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) { s_thr[i] = 0.0; s_wet[i] = 0.0; }
+  }
   const float* col = x + c0;
   const double* tcol = thr + c0;
+  // TableThr's row of step t, read through this kernel's __restrict__ pointers
   auto load = [&](int t, Vec<VEC>& r, double (&th)[VEC]) {
     r.load(col + (int64_t)t * ldx);
     load_thr<VEC>(tcol + (DOY ? (int64_t)(doy[t] - 1) : (int64_t)t) * rstride, th);
@@ -323,8 +329,14 @@ period_count_thr_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, con
   auto tally = [&](const Vec<VEC>& r, const double (&th)[VEC]) {
 #pragma unroll
     for (int i = 0; i < VEC; ++i) {
-      cnt[i] += cmp<OP>(r.v[i], fold_f64<OP>(th[i])) ? 1 : 0;
-      if constexpr (VALID) nv[i] += (r.v[i] == r.v[i]) ? 1 : 0;
+      if constexpr (SUMS) {
+        const float v = r.v[i];
+        s_thr[i] += cmp<OP>(v, fold_f64<OP>(th[i])) ? (double)v : 0.0;
+        s_wet[i] += cmp<OP>(v, wet) ? (double)v : 0.0;
+      } else {
+        cnt[i] += cmp<OP>(r.v[i], fold_f64<OP>(th[i])) ? 1 : 0;
+        if constexpr (VALID) nv[i] += (r.v[i] == r.v[i]) ? 1 : 0;
+      }
     }
   };
   int t = t0;
@@ -342,14 +354,24 @@ period_count_thr_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, con
     load(t, r, th);
     tally(r, th);
   }
-  store_vec<VEC>(out + (int64_t)p * C + c0, cnt);
-  if constexpr (VALID) store_vec<VEC>(valid + (int64_t)p * C + c0, nv);
+  if constexpr (SUMS) {
+    float a[VEC], b[VEC];
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) { a[i] = (float)s_thr[i]; b[i] = (float)s_wet[i]; }
+    store_vec<VEC>(out + (int64_t)p * C + c0, a);
+    store_vec<VEC>(valid + (int64_t)p * C + c0, b);
+  } else {
+    store_vec<VEC>(out + (int64_t)p * C + c0, cnt);
+    if constexpr (VALID) store_vec<VEC>(valid + (int64_t)p * C + c0, nv);
+  }
 }
 
 // 4 cells per thread when the layout allows 128-bit accesses, 1 otherwise; valid counts with a doy index only
-template <bool DOY>
+// (SUMS: both sums always)
+template <bool DOY, bool SUMS = false>
 int32_t launch_count_thr(const float* x, int64_t C, int64_t ldx, const int32_t* poff, int32_t P, const int16_t* doy,
-                         const double* thr, int64_t rstride, int32_t op, int32_t* out, int32_t* valid, cudaStream_t st) {
+                         const double* thr, int64_t rstride, int32_t op, std::conditional_t<SUMS, float, int32_t>* out,
+                         std::conditional_t<SUMS, float, int32_t>* valid, cudaStream_t st, float wet = 0.f) {
   const bool v4 = can_vec4(x, C, ldx, out, valid) && aligned16(thr) && rstride % 4 == 0;
   return dispatch_op(op, [&](auto OPC) -> int32_t {
     auto go = [&](auto VECC, auto VALC) -> int32_t {
@@ -357,15 +379,19 @@ int32_t launch_count_thr(const float* x, int64_t C, int64_t ldx, const int32_t* 
       const int64_t cblocks = (C + VEC * kThreads - 1) / (VEC * kThreads);
       XC_REQUIRE(cblocks <= 65535, "too many cells for one launch: tile the grid by latitude");
       const dim3 grid((unsigned)P, (unsigned)cblocks, 1);
-      period_count_thr_kernel<decltype(OPC)::value, VEC, decltype(VALC)::value, DOY><<<grid, kThreads, 0, st>>>(
-          x, C, ldx, poff, doy, thr, rstride, out, valid);
+      period_count_thr_kernel<decltype(OPC)::value, VEC, decltype(VALC)::value, DOY, SUMS>
+          <<<grid, kThreads, 0, st>>>(x, C, ldx, poff, doy, thr, rstride, out, valid, wet);
       return launch_status("period_count_thr_kernel");
     };
     auto go2 = [&](auto VECC) -> int32_t {
-      if constexpr (DOY) {
-        if (valid) return go(VECC, std::true_type{});
+      if constexpr (SUMS) {
+        return go(VECC, std::true_type{});
+      } else {
+        if constexpr (DOY) {
+          if (valid) return go(VECC, std::true_type{});
+        }
+        return go(VECC, std::false_type{});
       }
-      return go(VECC, std::false_type{});
     };
     return v4 ? go2(std::integral_constant<int, 4>{}) : go2(std::integral_constant<int, 1>{});
   });
@@ -575,16 +601,18 @@ extern "C" int32_t xc_period_count_f32(const float* x, int64_t T, int64_t C, int
 }
 
 namespace {
-template <int OP, int RED, bool FASTMAX>
+// v4: the layout of the threshold source allows 4 cells per thread as well
+template <int OP, int RED, bool FASTMAX, typename THR>
 int32_t launch_runstat(const float* x, int64_t T, int64_t C, int64_t ldx, const int32_t* poff, int32_t P,
-                       float t32, int32_t window, bool after, float* out, int32_t* valid, cudaStream_t st) {
-  const bool v4 = can_vec4(x, C, ldx, out, valid);
+                       THR thr, int32_t window, bool after, float* out, int32_t* valid, cudaStream_t st,
+                       bool thr_v4 = true) {
+  const bool v4 = can_vec4(x, C, ldx, out, valid) && thr_v4;
   auto go = [&](auto VECC, auto VALC, auto AFTC) -> int32_t {
     constexpr int VEC = decltype(VECC)::value;
     constexpr bool VAL = decltype(VALC)::value;
     constexpr bool AFT = decltype(AFTC)::value;
-    period_runstat_kernel<OP, RED, VEC, VAL, AFT, FASTMAX><<<grid_for(C, VEC, P), kThreads, 0, st>>>(
-        x, T, C, ldx, poff, t32, window, out, valid);
+    period_runstat_kernel<OP, RED, VEC, VAL, AFT, FASTMAX, THR><<<grid_for(C, VEC, P), kThreads, 0, st>>>(
+        x, T, C, ldx, poff, ThrParam<THR>::put(thr), window, out, valid);
     return launch_status("period_runstat_kernel");
   };
   auto go2 = [&](auto VECC) -> int32_t {
@@ -609,7 +637,7 @@ extern "C" int32_t xc_period_runstat_f32(const float* x, int64_t T, int64_t C, i
   return dispatch_op_nan(op, [&](auto OPC) -> int32_t {
     constexpr int OP = decltype(OPC)::value;
 #define XC_RS(RED, FAST) \
-  return launch_runstat<OP, RED, FAST>(x, T, C, ldx, period_offsets, P, t32, window, after, out, valid_count, st)
+  return launch_runstat<OP, RED, FAST>(x, T, C, ldx, period_offsets, P, ScalarThr{t32}, window, after, out, valid_count, st)
     switch (reducer) {
       case XC_RL_MAX:
         if (window == 1) { XC_RS(XC_RL_MAX, true); }
@@ -790,4 +818,59 @@ extern "C" int32_t xc_doy_threshold_count_f32(const float* x, int64_t T, int64_t
   XC_REQUIRE(T > 0 && C > 0 && ldx >= C && P > 0 && n_doy > 0, "bad shape");
   return launch_count_thr<true>(x, C, ldx, period_offsets, P, doy_index, table, C, op, out_count, valid_count,
                                 (cudaStream_t)stream);
+}
+
+extern "C" int32_t xc_doy_runstat_f32(const float* x, int64_t T, int64_t C, int64_t ldx,
+                                      const int32_t* period_offsets, int32_t P, const int16_t* doy_index,
+                                      const double* table, int32_t n_doy, int32_t op, int32_t reducer,
+                                      int32_t window, int32_t resample_before_rl, float* out, int32_t* valid_count,
+                                      void* stream) {
+  if (int32_t e = check_common(x, T, C, ldx, period_offsets, P, out)) return e;
+  XC_REQUIRE(doy_index != nullptr && table != nullptr, "null pointer argument");
+  XC_REQUIRE(n_doy > 0, "n_doy must be > 0, got %d", n_doy);
+  XC_REQUIRE(window >= 1, "window must be >= 1, got %d", window);
+  XC_REQUIRE(reducer >= XC_RL_MAX && reducer <= XC_RL_STD, "unknown run-length reducer %d", reducer);
+  XC_REQUIRE(op >= XC_OP_GT && op <= XC_OP_LE, "Operation `%d` not permitted for indice.", op);
+  const bool after = resample_before_rl == 0;
+  const bool thr_v4 = aligned16(table);
+  cudaStream_t st = (cudaStream_t)stream;
+  auto by_op = [&](auto OPC) -> int32_t {
+    constexpr int OP = decltype(OPC)::value;
+    const TableThr<OP, true> src{doy_index, table, C};
+#define XC_RS(RED) \
+  return launch_runstat<OP, RED, false>(x, T, C, ldx, period_offsets, P, src, window, after, out, valid_count, st, thr_v4)
+    switch (reducer) {
+      case XC_RL_MAX: XC_RS(XC_RL_MAX);
+      case XC_RL_MIN: XC_RS(XC_RL_MIN);
+      case XC_RL_SUM: XC_RS(XC_RL_SUM);
+      case XC_RL_COUNT: XC_RS(XC_RL_COUNT);
+      case XC_RL_MEAN: XC_RS(XC_RL_MEAN);
+      default: XC_RS(XC_RL_STD);
+    }
+#undef XC_RS
+  };
+  switch (op) {
+    case XC_OP_GT: return by_op(std::integral_constant<int, XC_OP_GT>{});
+    case XC_OP_LT: return by_op(std::integral_constant<int, XC_OP_LT>{});
+    case XC_OP_GE: return by_op(std::integral_constant<int, XC_OP_GE>{});
+    default: return by_op(std::integral_constant<int, XC_OP_LE>{});
+  }
+}
+
+extern "C" int32_t xc_period_sums_thr_f32(const float* x, int64_t T, int64_t C, int64_t ldx,
+                                          const int32_t* period_offsets, int32_t P, const int16_t* doy_index,
+                                          const double* thr, int64_t thr_rstride, int32_t op, double wet,
+                                          float* out_sum_thr, float* out_sum_wet, void* stream) {
+  if (int32_t e = check_common(x, T, C, ldx, period_offsets, P, out_sum_thr)) return e;
+  XC_REQUIRE(thr != nullptr && out_sum_wet != nullptr, "null pointer argument");
+  XC_REQUIRE(thr_rstride == 0 || thr_rstride >= C, "threshold row stride must be 0 (per cell) or >= C");
+  XC_REQUIRE(op == XC_OP_GT || op == XC_OP_GE, "Operation `%d` not permitted for indice.", op);
+  // the wet-day threshold is a Python float in the reference: compared in float32
+  const float w32 = (float)wet;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (doy_index)
+    return launch_count_thr<true, true>(x, C, ldx, period_offsets, P, doy_index, thr, thr_rstride, op, out_sum_thr,
+                                        out_sum_wet, st, w32);
+  return launch_count_thr<false, true>(x, C, ldx, period_offsets, P, nullptr, thr, thr_rstride, op, out_sum_thr,
+                                       out_sum_wet, st, w32);
 }

@@ -1,6 +1,8 @@
 // Run-length reducers, period edges of the runs and per-period statistics shared by the streaming kernels: one
 // copy of the rules.  The run-length code is __host__ __device__ so that a host build can test it.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 #define XC_RS_HD __host__ __device__ __forceinline__
@@ -65,6 +67,98 @@ __device__ __forceinline__ void stream_rows(const float* __restrict__ col, int64
     Vec<VEC> r;
     r.load(p);
     f(r);
+    p += ldx;
+  }
+}
+
+// ---- threshold sources ----------------------------------------------------------------------------------------------
+// What the element tests of a streaming kernel compare a cell's value with at step t.  A kernel loads the Row of a
+// step with load() next to its data and takes the float32 threshold of lane i with at().
+//   ScalarThr: one float32 threshold for every step and cell (nothing to load).
+//   TableThr<OP, DOY>: float64 thresholds thr[row(t) * rstride + c], row(t) = doy[t] - 1 (a day-of-year table,
+//     indices/_multivariate.py:1583-1590 with `resample_doy` as an index) or t (an array; rstride 0: one threshold
+//     per cell).  numpy compares float32 data with a float64 threshold in float64 (SURVEY.md A.1); each threshold
+//     is folded to the float32 with the same truth table (fold_f64), so that the element test is one float32
+//     compare.
+template <int VEC>
+__device__ __forceinline__ void load_thr(const double* p, double (&t)[VEC]) {
+  if constexpr (VEC == 4) {
+    const double2 a = *reinterpret_cast<const double2*>(p), b = *reinterpret_cast<const double2*>(p + 2);
+    t[0] = a.x; t[1] = a.y; t[2] = b.x; t[3] = b.y;
+  } else {
+    t[0] = *p;
+  }
+}
+
+struct ScalarThr {
+  float t;
+  template <int VEC>
+  struct Row {};
+  template <int VEC>
+  __device__ __forceinline__ void load(Row<VEC>&, int64_t, int) const {}
+  template <int VEC>
+  __device__ __forceinline__ float at(const Row<VEC>&, int) const { return t; }
+};
+
+// How a threshold source travels as a kernel parameter: a ScalarThr as its float, so that a kernel's scalar
+// instantiation keeps the parameter list (and code) it has without a source.
+template <typename SRC>
+struct ThrParam {
+  using type = SRC;
+  static __host__ __device__ __forceinline__ SRC put(const SRC& s) { return s; }
+  static __host__ __device__ __forceinline__ SRC get(const SRC& s) { return s; }
+};
+template <>
+struct ThrParam<ScalarThr> {
+  using type = float;
+  static __host__ __device__ __forceinline__ float put(const ScalarThr& s) { return s.t; }
+  static __host__ __device__ __forceinline__ ScalarThr get(float t) { return ScalarThr{t}; }
+};
+
+template <int OP, bool DOY>
+struct TableThr {
+  const int16_t* doy;
+  const double* thr;
+  int64_t rstride;
+  template <int VEC>
+  struct Row {
+    double v[VEC];
+  };
+  // cells c0 .. c0 + VEC - 1 of step t
+  template <int VEC>
+  __device__ __forceinline__ void load(Row<VEC>& r, int64_t c0, int t) const {
+    load_thr<VEC>(thr + c0 + (DOY ? (int64_t)(__ldg(doy + t) - 1) : (int64_t)t) * rstride, r.v);
+  }
+  template <int VEC>
+  __device__ __forceinline__ float at(const Row<VEC>& r, int i) const { return fold_f64<OP>(r.v[i]); }
+};
+
+// stream_rows with the threshold rows of `src` (for the cells from c0) loaded alongside: f(Vec, Row) for every t in
+// [t0, t1).  A ScalarThr source loads nothing: the loop is stream_rows'.
+template <int VEC, int UNROLL = 8, typename SRC, typename F>
+__device__ __forceinline__ void stream_rows_thr(const float* __restrict__ col, int64_t ldx, int t0, int t1,
+                                                const SRC& src, int64_t c0, F&& f) {
+  using Row = typename SRC::template Row<VEC>;
+  int t = t0;
+  const float* p = col + (int64_t)t0 * ldx;
+  for (; t + UNROLL <= t1; t += UNROLL) {
+    Vec<VEC> r[UNROLL];
+    Row th[UNROLL];
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      r[u].load(p + (int64_t)u * ldx);
+      src.load(th[u], c0, t + u);
+    }
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) f(r[u], th[u]);
+    p += (int64_t)UNROLL * ldx;
+  }
+  for (; t < t1; ++t) {
+    Vec<VEC> r;
+    Row th;
+    r.load(p);
+    src.load(th, c0, t);
+    f(r, th);
     p += ldx;
   }
 }

@@ -231,6 +231,77 @@ def doy_threshold_count(x2d, poff, doy_index, table2d, op_code, want_valid=False
     return out, valid
 
 
+def _doy_args(x2d, doy_index, n_rows):
+    doy_index = np.asarray(doy_index)
+    assert int(doy_index.max()) <= n_rows and int(doy_index.min()) >= 1
+    return dev_ints(doy_index, np.int16, x2d.device)
+
+
+def doy_runstat(x2d, poff, doy_index, table2d, op_code, reducer_code, window, resample_before_rl=True,
+                want_valid=False):
+    """Run statistic per period of ``float64(x[t]) op table[doy[t]-1]`` (xc_doy_runstat_f32): warm / cold spell
+    duration indices (indices/_multivariate.py:69-153, 1719-1795).  Returns ``(out, valid)`` as period_runstat."""
+    T, C = x2d.shape
+    P = len(poff) - 1
+    assert table2d.dtype == torch.float64 and table2d.is_contiguous() and table2d.shape[1] == C
+    doy_d = _doy_args(x2d, doy_index, table2d.shape[0])
+    poff_d = dev_ints(poff, np.int32, x2d.device)
+    out = torch.empty((P, C), dtype=torch.float32, device=x2d.device)
+    valid = torch.empty((P, C), dtype=torch.int32, device=x2d.device) if want_valid else None
+    check(load().xc_doy_runstat_f32(x2d.data_ptr(), T, C, x2d.stride(0), poff_d.data_ptr(), P, doy_d.data_ptr(),
+                                    table2d.data_ptr(), table2d.shape[0], op_code, reducer_code, int(window),
+                                    int(bool(resample_before_rl)), out.data_ptr(), _ptr(valid), current_stream_ptr()))
+    return out, valid
+
+
+def period_sums_thr(x2d, poff, op_code, thr2d, wet, doy_index=None, per_time=False):
+    """The two sums of fraction_over_precip_thresh (xc_period_sums_thr_f32): per period, the float32 sums of x
+    where ``float64(x) op thr`` and where ``x op float32(wet)``.  ``thr2d``: float64 (n_doy, C) with ``doy_index``,
+    else (T, C) with ``per_time`` or (1, C) (one threshold per cell)."""
+    T, C = x2d.shape
+    P = len(poff) - 1
+    assert thr2d.dtype == torch.float64 and thr2d.is_contiguous() and thr2d.shape[-1] == C
+    doy_d = None if doy_index is None else _doy_args(x2d, doy_index, thr2d.shape[0])
+    rstride = C if (doy_index is not None or per_time) else 0
+    poff_d = dev_ints(poff, np.int32, x2d.device)
+    s_thr = torch.empty((P, C), dtype=torch.float32, device=x2d.device)
+    s_wet = torch.empty((P, C), dtype=torch.float32, device=x2d.device)
+    check(load().xc_period_sums_thr_f32(x2d.data_ptr(), T, C, x2d.stride(0), poff_d.data_ptr(), P, _ptr(doy_d),
+                                        thr2d.data_ptr(), rstride, op_code, float(wet), s_thr.data_ptr(),
+                                        s_wet.data_ptr(), current_stream_ptr()))
+    return s_thr, s_wet
+
+
+def doy_count2(x1, x2, poff, doy_index, table1, table2, op1, op2):
+    """Days with ``x1 op1 table1[doy]`` and ``x2 op2 table2[doy]`` per period, float64 compares
+    (xc_doy_count2_f32): the compound percentile days (indices/_multivariate.py:162-416).  float32 (P, C)."""
+    T, C = x1.shape
+    assert x2.shape == x1.shape and x1.stride(0) == x2.stride(0)
+    for t in (table1, table2):
+        assert t.dtype == torch.float64 and t.is_contiguous() and t.shape == table1.shape and t.shape[1] == C
+    doy_d = _doy_args(x1, doy_index, table1.shape[0])
+    P = len(poff) - 1
+    poff_d = dev_ints(poff, np.int32, x1.device)
+    out = torch.empty((P, C), dtype=torch.float32, device=x1.device)
+    check(load().xc_doy_count2_f32(x1.data_ptr(), x2.data_ptr(), T, C, x1.stride(0), poff_d.data_ptr(), P,
+                                   doy_d.data_ptr(), table1.data_ptr(), table2.data_ptr(), table1.shape[0], op1, op2,
+                                   out.data_ptr(), current_stream_ptr()))
+    return out
+
+
+def period_range_stat(lo, hi, poff, stat_code, variability=False):
+    """Per-period statistic of ``hi - lo`` (float32, NaN skipped), or with ``variability`` the mean of its absolute
+    day-to-day change (xc_period_range_stat_f32): daily_temperature_range[_variability]."""
+    T, C = lo.shape
+    assert hi.shape == lo.shape and lo.stride(0) == hi.stride(0)
+    P = len(poff) - 1
+    poff_d = dev_ints(poff, np.int32, lo.device)
+    out = torch.empty((P, C), dtype=torch.float32, device=lo.device)
+    check(load().xc_period_range_stat_f32(lo.data_ptr(), hi.data_ptr(), T, C, lo.stride(0), poff_d.data_ptr(), P,
+                                          stat_code, int(bool(variability)), out.data_ptr(), current_stream_ptr()))
+    return out
+
+
 # ------------------------------------------------------------------------------------ host-buffer path
 def period_runstat_host(x_host, poff, op_code, thr, reducer_code, window, cmp_f64=False, want_valid=True,
                         workspace=None, out_host=None, valid_host=None):

@@ -67,19 +67,28 @@ def _percentile_table_count(da, per, code, freq, floor=None, want_valid=False):
     without the (lat, lon, time) float64 threshold array of the reference: the kernel indexes the per-doy table,
     converted to ``da``'s units and, with ``floor``, raised to ``floor`` where it is lower or NaN.  Returns the
     counts, the valid (non-NaN) counts when ``want_valid`` (else None) and ``(cell_shape, other, ta)`` of ``da``."""
-    import torch
-
     from . import device
-    from .calendar import adjust_table, table_on_device
     from .generic import _unwrap
 
     x2d, cell_shape, other, ta = _unwrap(da)
+    table, doy_idx = _doy_table(per, da, x2d, cell_shape, other, ta, floor)
+    cnt, valid = device.doy_threshold_count(x2d, ta.period_offsets(freq), doy_idx, table, code, want_valid=want_valid)
+    return cnt, valid, (cell_shape, other, ta)
+
+
+def _doy_table(per, da, x2d, cell_shape, other, ta, floor=None):
+    """``resample_doy(convert_units_to(per, da), da)`` as an index: the (n_doy, C) float64 device table of the
+    day-of-year array ``per`` in ``da``'s units (with ``floor``: raised to ``floor`` where it is lower or NaN,
+    ``per.where(per > floor, floor)``), adjusted to ``da``'s calendar (core/calendar.py:729-790), and the 1-based
+    table row of every time step."""
+    import torch
+
+    from .calendar import adjust_table, table_on_device
+
     table = _table_in_units_of(table_on_device(per, cell_shape, other, x2d.device), per, da)
     if floor is not None:
         table = torch.where(table > floor, table, torch.full_like(table, floor))
-    table, doy_idx = adjust_table(table, ta)
-    cnt, valid = device.doy_threshold_count(x2d, ta.period_offsets(freq), doy_idx, table, code, want_valid=want_valid)
-    return cnt, valid, (cell_shape, other, ta)
+    return adjust_table(table, ta)
 
 
 def _table_in_units_of(table, per, da):
@@ -134,6 +143,157 @@ def tg90p(tas, tas_per, freq="YS", bootstrap=False, op=">"):
 def tg10p(tas, tas_per, freq="YS", bootstrap=False, op="<"):
     """indices/_multivariate.py:1359-1414."""
     return _percentile_day_count(tas, tas_per, freq, bootstrap, op, ("<", "<="))
+
+
+# ------------------------------------------------------------------ the other day-of-year percentile indices
+def _spell_duration_index(da, per, window, freq, resample_before_rl, bootstrap, op, constrain, name):
+    """``compare(da, op, resample_doy(per, da))`` then ``rl.resample_and_rl(rl.windowed_run_count, window)``
+    (indices/_multivariate.py:69-153, 1719-1795) in one kernel that indexes the per-doy table."""
+    import numpy as np
+
+    from . import _lib, device
+    from .field import attrs_of
+    from .generic import _unwrap, _wrap_periods
+    if bootstrap:
+        raise NotImplementedError(f"{name}(bootstrap=True) is not supported by the xclim_b200 hot path")
+    code = _lib.op_code(op, constrain)
+    x2d, cell_shape, other, ta = _unwrap(da)
+    table, doy_idx = _doy_table(per, da, x2d, cell_shape, other, ta)
+    out, _ = device.doy_runstat(x2d, ta.period_offsets(freq), doy_idx, table, code, _lib.RL_REDUCERS["sum"],
+                                int(window), resample_before_rl)
+    attrs = attrs_of(da)
+    attrs["units"] = "d"
+    return _wrap_periods(da, out, cell_shape, other, ta, freq, attrs, dtype=np.float32)
+
+
+def warm_spell_duration_index(tasmax, tasmax_per, window=6, freq="YS", resample_before_rl=True, bootstrap=False,
+                              op=">"):
+    """Days inside spells of at least ``window`` days over the day-of-year percentile (ETCCDI WSDI) --
+    indices/_multivariate.py:1719-1795."""
+    return _spell_duration_index(tasmax, tasmax_per, window, freq, resample_before_rl, bootstrap, op, (">", ">="),
+                                 "warm_spell_duration_index")
+
+
+def cold_spell_duration_index(tasmin, tasmin_per, window=6, freq="YS", resample_before_rl=True, bootstrap=False,
+                              op="<"):
+    """Days inside spells of at least ``window`` days under the day-of-year percentile (ETCCDI CSDI) --
+    indices/_multivariate.py:69-153."""
+    return _spell_duration_index(tasmin, tasmin_per, window, freq, resample_before_rl, bootstrap, op, ("<", "<="),
+                                 "cold_spell_duration_index")
+
+
+def fraction_over_precip_thresh(pr, pr_per, thresh="1 mm/day", freq="YS", bootstrap=False, op=">"):
+    """Fraction of the wet-day precipitation that falls on days over a percentile (ETCCDI R95pTOT / R99pTOT) --
+    indices/_multivariate.py:1238-1297.  ``pr_per`` has a ``dayofyear`` dimension (one threshold per day of
+    the year) or none (one threshold per cell); ``tp = pr_per.where(pr_per > thresh, thresh)`` is applied on
+    the device and both sums come from one read of ``pr``."""
+    import numpy as np
+
+    from . import _lib, device
+    from .field import attrs_of, dims_of
+    from .generic import _array_threshold, _unwrap, _wrap_periods
+    if bootstrap:
+        raise NotImplementedError("fraction_over_precip_thresh(bootstrap=True) is not supported by the xclim_b200 "
+                                  "hot path")
+    code = _lib.op_code(op, (">", ">="))
+    thr = threshold_in_units_of(thresh, pr) if isinstance(thresh, str) else float(thresh)
+    x2d, cell_shape, other, ta = _unwrap(pr)
+    poff = ta.period_offsets(freq)
+    if "dayofyear" in dims_of(pr_per):
+        table, doy_idx = _doy_table(pr_per, pr, x2d, cell_shape, other, ta, floor=thr)
+        s_thr, s_wet = device.period_sums_thr(x2d, poff, code, table, thr, doy_index=doy_idx)
+    else:
+        import torch
+        arr = _array_threshold(pr_per, pr, cell_shape, other, x2d)
+        if arr is None:
+            raise ValueError("pr_per must be an array with a `dayofyear` dimension or one value per cell")
+        tp = _table_in_units_of(arr[0], pr_per, pr)
+        tp = torch.where(tp > thr, tp, torch.full_like(tp, thr)).contiguous()
+        s_thr, s_wet = device.period_sums_thr(x2d, poff, code, tp, thr, per_time=arr[1])
+    attrs = attrs_of(pr)
+    attrs["units"] = ""
+    return _wrap_periods(pr, s_thr / s_wet, cell_shape, other, ta, freq, attrs, dtype=np.float32)
+
+
+def _compound_days(tas, pr, tas_per, pr_per, freq, tas_op, pr_op):
+    """``(tas op tas_per[doy]) & (pr op pr_per[doy])`` counted per period (indices/_multivariate.py:162-416), both
+    compares in float64 against the per-doy tables, in one kernel."""
+    import numpy as np
+
+    from . import _lib, device
+    from .field import attrs_of
+    from .generic import _unwrap, _wrap_periods
+    x1, cell_shape, other, ta = _unwrap(tas)
+    x2, cs2, _, ta2 = _unwrap(pr)
+    if cs2 != cell_shape or len(ta2) != len(ta):
+        raise ValueError("the two variables must share the same grid and time axis")
+    t1, d1 = _doy_table(tas_per, tas, x1, cell_shape, other, ta)
+    t2, d2 = _doy_table(pr_per, pr, x1, cell_shape, other, ta)
+    d1, d2 = np.asarray(d1), np.asarray(d2)
+    if not np.array_equal(d1, d2):
+        # one table is on the data's calendar (indexed by day of year), the other was interpolated onto the doy
+        # range of the data (indexed from its first day): take the same rows of the first
+        lo = int(ta.doy.min())
+        t1, t2 = (t1[lo - 1:lo - 1 + t2.shape[0]].contiguous(), t2) if t1.shape[0] == ta.max_doy else \
+            (t1, t2[lo - 1:lo - 1 + t1.shape[0]].contiguous())
+        d1 = np.asarray(ta.doy) - lo + 1
+    out = device.doy_count2(x1, x2, ta.period_offsets(freq), d1, t1, t2, _lib.OPS[tas_op], _lib.OPS[pr_op])
+    attrs = attrs_of(tas)
+    attrs["units"] = "d"
+    return _wrap_periods(tas, out, cell_shape, other, ta, freq, attrs, dtype=np.int64)
+
+
+def cold_and_dry_days(tas, pr, tas_per, pr_per, freq="YS"):
+    """Days colder than the ``tas_per`` and drier than the ``pr_per`` day-of-year percentiles --
+    indices/_multivariate.py:162-223."""
+    return _compound_days(tas, pr, tas_per, pr_per, freq, "<", "<")
+
+
+def warm_and_dry_days(tas, pr, tas_per, pr_per, freq="YS"):
+    """indices/_multivariate.py:226-289."""
+    return _compound_days(tas, pr, tas_per, pr_per, freq, ">", "<")
+
+
+def warm_and_wet_days(tas, pr, tas_per, pr_per, freq="YS"):
+    """indices/_multivariate.py:292-355."""
+    return _compound_days(tas, pr, tas_per, pr_per, freq, ">", ">")
+
+
+def cold_and_wet_days(tas, pr, tas_per, pr_per, freq="YS"):
+    """indices/_multivariate.py:358-416."""
+    return _compound_days(tas, pr, tas_per, pr_per, freq, "<", ">")
+
+
+def _temperature_range(tasmin, tasmax, freq, op, variability, name):
+    from . import _lib, device
+    from .field import attrs_of
+    from .generic import _unwrap, _wrap_periods
+    from .units import units_of
+    if units_of(tasmax) != units_of(tasmin):
+        raise NotImplementedError(f"{name}: give tasmax and tasmin in the same units")
+    if not isinstance(op, str) or op not in _lib.STATS or op in ("count", "integral"):
+        raise NotImplementedError(f"resample op {op!r} is not supported by the xclim_b200 hot path")
+    lo, cell_shape, other, ta = _unwrap(tasmin)
+    hi, cs2, _, ta2 = _unwrap(tasmax)
+    if cs2 != cell_shape or len(ta2) != len(ta):
+        raise ValueError("the two variables must share the same grid and time axis")
+    out = device.period_range_stat(lo, hi, ta.period_offsets(freq), _lib.STATS[op], variability)
+    u = attrs_of(tasmax).get("units", "")
+    attrs = {**attrs_of(tasmax), "units": {"degC": "K", "°C": "K", "C": "K"}.get(u, u),
+             "units_metadata": "temperature: difference"}
+    return _wrap_periods(tasmax, out, cell_shape, other, ta, freq, attrs)
+
+
+def daily_temperature_range(tasmin, tasmax, freq="YS", op="mean"):
+    """Statistic of the daily temperature range ``tasmax - tasmin`` per period (ETCCDI DTR for ``op="mean"``) --
+    indices/_multivariate.py:514-557 (both inputs in the same units; the result is a temperature difference)."""
+    return _temperature_range(tasmin, tasmax, freq, op, False, "daily_temperature_range")
+
+
+def daily_temperature_range_variability(tasmin, tasmax, freq="YS"):
+    """Mean absolute day-to-day change of the daily temperature range -- indices/_multivariate.py:561-598.  The
+    change into a period's first day is that period's; the series' first day has none."""
+    return _temperature_range(tasmin, tasmax, freq, "mean", True, "daily_temperature_range_variability")
 
 
 # ------------------------------------------------------------------ rolling / spell families
