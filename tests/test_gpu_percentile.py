@@ -79,12 +79,13 @@ def test_percentile_doy_standard_calendar_and_366(cuda):
     got = xcal.percentile_doy(da, window=5, per=90.0)
     exp = O.percentile_doy(x, da.time.year, da.time.doy, 5, 90.0)[:, 0]
     assert _table(got).shape[0] == 366
-    np.testing.assert_allclose(_table(got), exp, rtol=RTOL)
+    # the re-interpolation (xc_doy_interp_f64) repeats np.interp's operations: bit-identical
+    np.testing.assert_array_equal(_table(got), exp)
     # partial first/last years (series not starting on Jan 1st)
     da2 = make_field(x[100:-50], "1999-04-11", calendar="standard", units="K")
     got2 = xcal.percentile_doy(da2, window=5, per=10.0)
     exp2 = O.percentile_doy(x[100:-50], da2.time.year, da2.time.doy, 5, 10.0)[:, 0]
-    np.testing.assert_allclose(_table(got2), exp2, rtol=RTOL, equal_nan=True)
+    np.testing.assert_array_equal(_table(got2), exp2)
 
 
 def test_percentile_doy_reference_known_answers(cuda):
@@ -226,14 +227,15 @@ def test_percentile_doy_mid_percentiles_selection_kernel(cuda, calendar, years, 
     np.testing.assert_array_equal(g, exp)
 
 
-@pytest.mark.parametrize("years", [30, 31, 32])
-@pytest.mark.parametrize("per", [90.0, 10.0])
+@pytest.mark.parametrize("per,years", [(90.0, 30), (90.0, 31), (92.0, 32), (10.0, 30), (10.0, 31), (8.0, 32)])
 def test_percentile_doy_tma_path(cuda, years, per, monkeypatch):
     """The TMA-fed window-5 kernel (30..32 uniform years, ldx % 4 == 0): bit-exact vs the oracle and vs
     the lane-by-lane kernel, with NaNs, infinities of both signs (the FADD NaN probe's false positive),
     cells beyond the last full 128-cell tile, windows that reach into the neighbouring year, and samples
-    whose interpolation meets infinities or overflows (NaN lerp -> the sample maximum)."""
+    whose interpolation meets infinities or overflows (NaN lerp -> the sample maximum).  32 years take
+    the 92nd / 8th percentile: the 90th / 10th need 17 order statistics there, beyond the TMA kernel's 16."""
     import torch
+    from pdoy_dispatch import kernels
     from xclim_b200 import device
     rng = np.random.default_rng(100 + years)
     L, T = 365, years * 365
@@ -249,6 +251,9 @@ def test_percentile_doy_tma_path(cuda, years, per, monkeypatch):
     yidx = (np.arange(T) // L).astype(np.int16)
     xd = torch.from_numpy(x.reshape(T, -1)).cuda()
     assert xd.shape[1] % 4 == 0
+    C = xd.shape[1]
+    assert kernels(doy, yidx, L, years, 5, [per], C) == {f"w5t<{years - 16}>"}
+    assert kernels(doy, yidx, L, years, 5, [per], C, no_tma=True) == {"w5p<16, false>"}
     monkeypatch.delenv("XCLIM_B200_NO_TMA", raising=False)
     a = device.percentile_doy(xd, doy, yidx, L, years, 5, [per], 1 / 3, 1 / 3)
     monkeypatch.setenv("XCLIM_B200_NO_TMA", "1")
