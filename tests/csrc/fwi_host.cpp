@@ -5,6 +5,8 @@
 // with host pointers and a plain loop over the cells in place of the CUDA grid.  tests/test_fire_host_core.py
 // checks it against the oracle and the reference fixtures, so that the arithmetic and the state machine of
 // the kernel are verified where no GPU is available.  Nothing in xclim_b200/ loads this library.
+#include <cstddef>
+
 #include "../../xclim_b200/csrc/fwi_core.cuh"
 
 static const double h_day_lengths[60] = XC_FWI_DAY_LENGTHS;
@@ -47,3 +49,10 @@ extern "C" int32_t fwi_host_elementwise_f32(int32_t kind, const float* a, const 
 
 // test hook: numpy's float32 mean of a ring (newest value at `head`)
 extern "C" float fwi_host_np_mean(const float* ring, int32_t n, int32_t head) { return xc::fwi::np_mean_f32(ring, n, head); }
+
+// test hook: the layout of XcFwiParams that the bindings must reproduce
+extern "C" void fwi_host_params_layout(int64_t* out) {
+  out[0] = sizeof(XcFwiParams);
+  out[1] = offsetof(XcFwiParams, snow_min_cover_frac);
+  out[2] = offsetof(XcFwiParams, in_scale);
+}

@@ -1,6 +1,7 @@
 // Host build of the evapotranspiration device code (xclim_b200/csrc/pet_core.cuh) for the CPU test-suite: the
 // element loop of pet_daily_kernel and the cell loop of pet_monthly_kernel (pet.cu) over host arrays, compiled with
 // g++ -ffp-contract=off, behind the argument checks of the C-ABI entry points.
+#include <stddef.h>
 #include <stdint.h>
 
 #include "../../xclim_b200/csrc/pet_core.cuh"
@@ -38,6 +39,13 @@ int32_t pet_host_monthly(const float* const* inputs, int64_t T, int64_t C, int64
   if (check_args(a, true)) return -1;
   for (int64_t c = 0; c < C; ++c) monthly_cell(a, c);
   return 0;
+}
+
+// the layout of XcPetParams that the bindings must reproduce
+void pet_host_params_layout(int64_t* out) {
+  out[0] = sizeof(XcPetParams);
+  out[1] = offsetof(XcPetParams, in_scale);
+  out[2] = offsetof(XcPetParams, peta);
 }
 
 }  // extern "C"

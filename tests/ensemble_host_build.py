@@ -1,39 +1,21 @@
 """TEST INFRASTRUCTURE: build and bind the host build of the ensemble robustness device code
 (tests/csrc/ensemble_host.cpp over xclim_b200/csrc/ensemble_core.cuh)."""
 import ctypes
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-_lib = None
+import host_build
+
 _vp, _i64, _i32, _f64 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_double
+SIGNATURES = {
+    "ens_host_stdtr": (None, [_vp, _vp, _i64, _vp]),
+    "ens_host_ttest_1samp_p": (_f64, [_i32, _f64, _f64, _f64]),
+    "ens_host_welch_ttest_p": (_f64, [_i32, _f64, _f64, _i32, _f64, _f64]),
+}
 
 
 def load():
-    global _lib
-    if _lib is None:
-        out = os.path.join(tempfile.gettempdir(), f"libxclim_b200_ensemble_host_{os.getuid()}.so")
-        src = os.path.join(HERE, "csrc", "ensemble_host.cpp")
-        csrc = os.path.join(ROOT, "xclim_b200", "csrc")
-        deps = [src, os.path.join(csrc, "ensemble_core.cuh"), os.path.join(csrc, "stdindex_core.cuh"),
-                os.path.join(csrc, "npsum.cuh"), os.path.join(ROOT, "include", "xclim_b200.h")]
-        if not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-            tmp = out + f".{os.getpid()}.tmp"
-            cmd = ["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", src, "-o", tmp]
-            subprocess.run(cmd, check=True, capture_output=True, text=True)
-            os.replace(tmp, out)
-        lib = ctypes.CDLL(out)
-        lib.ens_host_stdtr.argtypes = [_vp, _vp, _i64, _vp]
-        lib.ens_host_ttest_1samp_p.restype = _f64
-        lib.ens_host_ttest_1samp_p.argtypes = [_i32, _f64, _f64, _f64]
-        lib.ens_host_welch_ttest_p.restype = _f64
-        lib.ens_host_welch_ttest_p.argtypes = [_i32, _f64, _f64, _i32, _f64, _f64]
-        _lib = lib
-    return _lib
+    return host_build.load("ensemble", "ensemble_host.cpp", signatures=SIGNATURES)
 
 
 def _p(a):

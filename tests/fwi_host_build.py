@@ -1,47 +1,25 @@
 """TEST INFRASTRUCTURE: build and bind the host build of the fire-weather device code (tests/csrc/fwi_host.cpp)."""
 import ctypes
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-_lib = None
+import host_build
+from xclim_b200 import _lib as L
 
-
-class XcFwiParams(ctypes.Structure):
-    """include/xclim_b200.h XcFwiParams (the product's own binding is xclim_b200/_lib.py)."""
-    _fields_ = ([(n, ctypes.c_int32) for n in ("season_mode", "overwintering", "dry_start", "initial_start_up",
-                                              "temp_condition_days", "snow_condition_days", "snow_cover_days")]
-                + [(n, ctypes.c_float) for n in ("temp_start_thresh", "temp_end_thresh", "snow_thresh", "prec_thresh",
-                                                 "snow_min_mean_depth", "dc_start", "dmc_start", "ffmc_start",
-                                                 "dc_dry_factor", "dmc_dry_factor")]
-                + [(n, ctypes.c_double) for n in ("snow_min_cover_frac", "carry_over_fraction",
-                                                  "wetting_efficiency_fraction", "min_dc")]
-                + [("in_scale", ctypes.c_float * 5), ("in_offset", ctypes.c_float * 5)])
+_vp, _i64, _i32, _f64 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_double
+SIGNATURES = {
+    "fwi_host_last_error": (ctypes.c_char_p, []),
+    "fwi_host_f32": (_i32, [_vp] * 12 + [_i64, _i64, _i64, _vp] + [_vp] * 9),
+    "fwi_host_elementwise_f32": (_i32, [_i32, _vp, _vp, _i64, _f64, _f64, _f64, _vp]),
+    "fwi_host_np_mean": (ctypes.c_float, [_vp, _i32, _i32]),
+    "fwi_host_params_layout": (None, [ctypes.POINTER(_i64)]),
+}
 
 
 def load():
-    global _lib
-    if _lib is None:
-        out = os.path.join(tempfile.gettempdir(), f"libxclim_b200_fwi_host_{os.getuid()}.so")
-        src = os.path.join(HERE, "csrc", "fwi_host.cpp")
-        deps = [src, os.path.join(ROOT, "xclim_b200", "csrc", "fwi_core.cuh"), os.path.join(ROOT, "include", "xclim_b200.h")]
-        if not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-            inc = "/usr/local/cuda/include"
-            cmd = ["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", src, "-o", out]
-            if os.path.isdir(inc):
-                cmd[1:1] = ["-I" + inc]
-            subprocess.run(cmd, check=True, capture_output=True, text=True)
-        _lib = ctypes.CDLL(out)
-        _lib.fwi_host_last_error.restype = ctypes.c_char_p
-    return _lib
+    return host_build.load("fwi", "fwi_host.cpp", signatures=SIGNATURES)
 
 
-SEASON = {None: 0, "mask": 1, "WF93": 2, "LA08": 3, "GFWED": 4}
-DRY = {None: 0, "CFS": 1, "GFWED": 2, "GFWED+SNOW": 3}
 DEFAULTS = dict(temp_start_thresh=12.0, temp_end_thresh=5.0, snow_thresh=0.01, temp_condition_days=3,
                 snow_condition_days=3, carry_over_fraction=0.75, wetting_efficiency_fraction=0.75, dc_start=15,
                 dmc_start=6, ffmc_start=85, prec_thresh=1.0, dc_dry_factor=5, dmc_dry_factor=2, snow_cover_days=60,
@@ -51,8 +29,9 @@ DEFAULTS = dict(temp_start_thresh=12.0, temp_end_thresh=5.0, snow_thresh=0.01, t
 def params(season_method=None, overwintering=False, dry_start=None, initial_start_up=True, **kw):
     p = dict(DEFAULTS)
     p.update(kw)
-    P = XcFwiParams()
-    P.season_mode, P.overwintering, P.dry_start = SEASON[season_method], int(overwintering), DRY[dry_start]
+    P = L.FwiParams()
+    P.season_mode, P.overwintering = L.FWI_SEASONS[season_method], int(overwintering)
+    P.dry_start = L.FWI_DRY_STARTS[dry_start]
     P.initial_start_up = int(initial_start_up)
     for k in ("temp_condition_days", "snow_condition_days", "snow_cover_days"):
         setattr(P, k, int(p[k]))
@@ -114,8 +93,7 @@ def elementwise(kind, a, b=None, p=(0.0, 0.0, 0.0)):
     a = np.ascontiguousarray(a, dtype=np.float32)
     bb = None if b is None else np.ascontiguousarray(np.broadcast_to(b, a.shape), dtype=np.float32)
     out = np.empty_like(a)
-    code = {"ISI": 0, "BUI": 1, "FWI": 2, "DSR": 3, "OWDC": 4}[kind]
-    lib.fwi_host_elementwise_f32(ctypes.c_int32(code), a.ctypes.data_as(ctypes.c_void_p),
+    lib.fwi_host_elementwise_f32(ctypes.c_int32(L.FWI_ELEMENTWISE[kind]), a.ctypes.data_as(ctypes.c_void_p),
                                  None if bb is None else bb.ctypes.data_as(ctypes.c_void_p), ctypes.c_int64(a.size),
                                  ctypes.c_double(p[0]), ctypes.c_double(p[1]), ctypes.c_double(p[2]),
                                  out.ctypes.data_as(ctypes.c_void_p))

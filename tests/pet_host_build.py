@@ -2,38 +2,22 @@
 (tests/csrc/pet_host.cpp over xclim_b200/csrc/pet_core.cuh), behind the argument lists of device.pet_daily and
 device.pet_monthly with numpy arrays in place of device tensors."""
 import ctypes
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
+import host_build
 from xclim_b200 import _lib as L
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-_lib = None
 _vp, _i64, _i32 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32
+SIGNATURES = {
+    "pet_host_daily": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _vp]),
+    "pet_host_monthly": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp]),
+    "pet_host_params_layout": (None, [ctypes.POINTER(_i64)]),
+}
 
 
 def load():
-    global _lib
-    if _lib is None:
-        out = os.path.join(tempfile.gettempdir(), f"libxclim_b200_pet_host_{os.getuid()}.so")
-        src = os.path.join(HERE, "csrc", "pet_host.cpp")
-        deps = [src, os.path.join(ROOT, "include", "xclim_b200.h"), os.path.join(ROOT, "xclim_b200", "csrc", "pet_core.cuh")]
-        if not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-            tmp = out + f".{os.getpid()}.tmp"
-            cmd = ["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", src, "-o", tmp]
-            subprocess.run(cmd, check=True, capture_output=True, text=True)
-            os.replace(tmp, out)
-        lib = ctypes.CDLL(out)
-        lib.pet_host_daily.restype = _i32
-        lib.pet_host_daily.argtypes = [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _vp]
-        lib.pet_host_monthly.restype = _i32
-        lib.pet_host_monthly.argtypes = [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp]
-        _lib = lib
-    return _lib
+    return host_build.load("pet", "pet_host.cpp", signatures=SIGNATURES)
 
 
 def _p(a):

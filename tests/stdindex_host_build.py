@@ -1,44 +1,23 @@
 """TEST INFRASTRUCTURE: build and bind the host build of the standardized-index device code
 (tests/csrc/stdindex_host.cpp over xclim_b200/csrc/stdindex_core.cuh)."""
 import ctypes
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-_lib = None
-_vp, _i64, _i32, _f64 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_double
+import host_build
+from xclim_b200 import _lib as L
 
-DISTS = {"gamma": 0, "fisk": 1, "lognorm": 2}
-METHODS = {"APP": 0, "ML": 1}
+_vp, _i64, _i32, _f64 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_double
+SIGNATURES = {
+    "si_host_np_mean": (ctypes.c_float, [_vp, _i32]),
+    "si_host_gamma_ml_shape": (_f64, [_f64, _f64, _f64, _vp]),
+    "si_host_fit": (_i32, [_vp, _i64, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _f64, _vp, _vp, _vp, _vp]),
+    "si_host_apply": (None, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _i32, _i32, _f64, _f64, _f64, _vp]),
+}
 
 
 def load():
-    global _lib
-    if _lib is None:
-        out = os.path.join(tempfile.gettempdir(), f"libxclim_b200_stdindex_host_{os.getuid()}.so")
-        src = os.path.join(HERE, "csrc", "stdindex_host.cpp")
-        csrc = os.path.join(ROOT, "xclim_b200", "csrc")
-        deps = [src, os.path.join(csrc, "stdindex_core.cuh"), os.path.join(csrc, "npsum.cuh"),
-                os.path.join(ROOT, "include", "xclim_b200.h")]
-        if not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-            tmp = out + f".{os.getpid()}.tmp"
-            cmd = ["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", src, "-o", tmp]
-            subprocess.run(cmd, check=True, capture_output=True, text=True)
-            os.replace(tmp, out)
-        lib = ctypes.CDLL(out)
-        lib.si_host_np_mean.restype = ctypes.c_float
-        lib.si_host_np_mean.argtypes = [_vp, _i32]
-        lib.si_host_gamma_ml_shape.restype = _f64
-        lib.si_host_gamma_ml_shape.argtypes = [_f64, _f64, _f64, _vp]
-        lib.si_host_fit.restype = _i32
-        lib.si_host_fit.argtypes = [_vp, _i64, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _f64, _vp, _vp, _vp, _vp]
-        lib.si_host_apply.argtypes = [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _i32, _i32, _f64, _f64, _f64, _vp]
-        _lib = lib
-    return _lib
+    return host_build.load("stdindex", "stdindex_host.cpp", signatures=SIGNATURES)
 
 
 def _p(a):
@@ -101,8 +80,8 @@ def fit(y, group_of_step, G, dist, method, zero_inflated, floc, cal=slice(None))
     nz = np.full((G, C), -1, np.int32)
     nn = np.full((G, C), -1, np.int32)
     ws = np.empty(max_n * C, np.float32)
-    st = load().si_host_fit(_p(y), C, C, _p(goff), _p(steps), G, DISTS[dist], METHODS[method], int(zero_inflated),
-                            float(floc), _p(params), _p(nz), _p(nn), _p(ws))
+    st = load().si_host_fit(_p(y), C, C, _p(goff), _p(steps), G, L.SI_DISTS[dist], L.SI_METHODS[method],
+                            int(zero_inflated), float(floc), _p(params), _p(nz), _p(nn), _p(ws))
     return params, (nz if zero_inflated else None), (nn if zero_inflated else None), st
 
 
@@ -115,6 +94,6 @@ def apply(y, group_of_step, params, dist, n_zeros=None, n_notnull=None, interp=1
     nz = np.ascontiguousarray(n_zeros if zi else np.zeros(1), dtype=np.int32)
     nn = np.ascontiguousarray(n_notnull if zi else np.zeros(1), dtype=np.int32)
     out = np.empty((T, C))
-    load().si_host_apply(_p(y), T, C, C, _p(gos), _p(params), _p(nz), _p(nn), DISTS[dist], int(zi), float(interp),
+    load().si_host_apply(_p(y), T, C, C, _p(gos), _p(params), _p(nz), _p(nn), L.SI_DISTS[dist], int(zi), float(interp),
                          float(alpha), float(beta), _p(out))
     return out

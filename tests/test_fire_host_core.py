@@ -60,15 +60,14 @@ def test_argument_checks_of_the_library():
 
 
 def test_parameter_struct_layouts_agree():
-    """The product's ctypes struct (xclim_b200/_lib.py) and the one the host build was driven with lay
-    XcFwiParams out identically (144 bytes; the doubles 8-aligned after 17 4-byte fields)."""
+    """The product's ctypes struct (xclim_b200/_lib.py) lays XcFwiParams out as the C compiler does (144 bytes;
+    the doubles 8-aligned after 17 4-byte fields)."""
     import ctypes
 
     from xclim_b200 import _lib
-    assert ctypes.sizeof(_lib.FwiParams) == ctypes.sizeof(hb.XcFwiParams) == 144
-    for (n1, _), (n2, _) in zip(_lib.FwiParams._fields_, hb.XcFwiParams._fields_):
-        assert n1 == n2 and getattr(_lib.FwiParams, n1).offset == getattr(hb.XcFwiParams, n2).offset
-    assert _lib.FwiParams.snow_min_cover_frac.offset == 72 and _lib.FwiParams.in_scale.offset == 104
+    P, c = _lib.FwiParams, (ctypes.c_int64 * 3)()
+    hb.load().fwi_host_params_layout(c)          # sizeof, offsetof snow_min_cover_frac, offsetof in_scale
+    assert (ctypes.sizeof(P), P.snow_min_cover_frac.offset, P.in_scale.offset) == tuple(c) == (144, 72, 104)
 
 
 def test_elementwise_functions_of_the_host_build(golden):  # noqa: F811

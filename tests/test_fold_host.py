@@ -4,38 +4,27 @@
 array-threshold counts on the device and the scalar thresholds of every ``cmp_f64`` entry point on the host."""
 import ctypes
 import operator
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-OPS = {">": (0, operator.gt), "<": (1, operator.lt), ">=": (2, operator.ge), "<=": (3, operator.le),
-       "==": (4, operator.eq), "!=": (5, operator.ne)}
+import host_build
+from xclim_b200 import _lib
+
+#: the operators with the numpy comparison each must reproduce
+OPS = {">": operator.gt, "<": operator.lt, ">=": operator.ge, "<=": operator.le, "==": operator.eq, "!=": operator.ne}
 
 
 @pytest.fixture(scope="module")
 def fold_lib():
-    from xclim_b200 import _build
-    out = os.path.join(tempfile.gettempdir(), f"libxclim_b200_fold_host_{os.getuid()}.so")
-    src = os.path.join(HERE, "csrc", "fold_host.cu")
-    deps = [src, os.path.join(ROOT, "xclim_b200", "csrc", "common.cuh"), os.path.join(ROOT, "include", "xclim_b200.h")]
-    if not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-        cmd = [_build._nvcc(), "-O2", "-std=c++17", *_build.ARCH_FLAGS, "-Xcompiler", "-fPIC", "-shared", src,
-               "-o", out]
-        subprocess.run(cmd, check=True, capture_output=True, text=True)
-    lib = ctypes.CDLL(out)
-    lib.fold_host_f64.restype = ctypes.c_int32
-    return lib
+    sig = (ctypes.c_int32, [ctypes.c_int32, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p])
+    return host_build.load("fold", "fold_host.cu", nvcc=True, signatures={"fold_host_f64": sig})
 
 
 def fold(lib, op, t):
     t = np.ascontiguousarray(t, dtype=np.float64)
     out = np.empty(t.shape, np.float32)
-    assert lib.fold_host_f64(ctypes.c_int32(OPS[op][0]), t.ctypes.data_as(ctypes.c_void_p), ctypes.c_int64(t.size),
+    assert lib.fold_host_f64(_lib.OPS[op], t.ctypes.data_as(ctypes.c_void_p), t.size,
                              out.ctypes.data_as(ctypes.c_void_p)) == 0
     return out
 
@@ -63,7 +52,7 @@ def edges():
 def test_fold_gives_the_float64_compare_for_every_float32(fold_lib, op):
     x, t = edges()
     f = fold(fold_lib, op, t)
-    fn = OPS[op][1]
+    fn = OPS[op]
     with np.errstate(invalid="ignore"):
         got = fn(x[:, None], f[None, :])
         exp = fn(x[:, None].astype(np.float64), t[None, :])

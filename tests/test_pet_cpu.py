@@ -156,6 +156,14 @@ def test_host_build_monthly_group_longer_than_a_year_is_nan():
     assert M > 12 and np.isnan(out).all()
 
 
+def test_parameter_struct_layout_agrees():
+    """The product's ctypes struct (xclim_b200/_lib.py) lays XcPetParams out as the C compiler does (128 bytes;
+    the doubles after the two ints and the 2 x 11 floats)."""
+    P, c = _lib.PetParams, (ctypes.c_int64 * 3)()
+    H.load().pet_host_params_layout(c)           # sizeof, offsetof in_scale, offsetof peta
+    assert (ctypes.sizeof(P), P.in_scale.offset, P.peta.offset) == tuple(c) == (128, 8, 96)
+
+
 # ------------------------------------------------------------------------------------ host layer
 def _stand_in_daily(inputs, table, lat_index, params):
     np_in = [None if x is None else x.numpy() for x in inputs]

@@ -5,38 +5,25 @@ close.  Every boolean series of 12 steps, against the oracle's ``resample_and_rl
 and periods that leave steps before and after them, both ``resample_before_rl``, windows 1-4, all six reducers and
 every accumulator form the kernels instantiate."""
 import ctypes
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
+import host_build
 from oracle import xclim_oracle as O
+from xclim_b200._lib import RL_REDUCERS as REDUCERS
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 T = 12
 MASK = ((np.arange(2 ** T)[None, :] >> np.arange(T)[:, None]) & 1).astype(bool)   # (T, 4096): every series
-REDUCERS = {"max": 0, "min": 1, "sum": 2, "count": 3, "mean": 4, "std": 5}
 POFFS = [[0, 12], [0, 5, 12], [0, 1, 6, 7, 12], [2, 5, 9]]
 FORMS = {"fixed": 0, "any": 1, "running": 2}
 
 
 @pytest.fixture(scope="module")
 def runs_lib():
-    from xclim_b200 import _build
-    out = os.path.join(tempfile.gettempdir(), f"libxclim_b200_runs_host_{os.getuid()}.so")
-    src = os.path.join(HERE, "csrc", "runs_host.cu")
-    deps = [src, os.path.join(ROOT, "include", "xclim_b200.h")] + \
-        [os.path.join(ROOT, "xclim_b200", "csrc", h) for h in ("runstat.cuh", "common.cuh")]
-    if not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps):
-        cmd = [_build._nvcc(), "-O2", "-std=c++17", *_build.ARCH_FLAGS, "-Xcompiler", "-fPIC", "-shared", src,
-               "-o", out]
-        subprocess.run(cmd, check=True, capture_output=True, text=True)
-    lib = ctypes.CDLL(out)
-    lib.runs_host.restype = ctypes.c_int32
-    return lib
+    _vp, _i32 = ctypes.c_void_p, ctypes.c_int32
+    sig = (_i32, [_vp, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp])
+    return host_build.load("runs", "runs_host.cu", nvcc=True, signatures={"runs_host": sig})
 
 
 def runs(lib, poff, before, reducer, window, form):

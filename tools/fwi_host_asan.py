@@ -1,19 +1,17 @@
 """The host build of the fire-weather device code under AddressSanitizer + UBSan (every fixture case and the
 longest rings).  Run from the repository root:
 
-    g++ -O1 -g -std=c++17 -ffp-contract=off -fPIC -shared -fsanitize=address,undefined -fno-omit-frame-pointer \\
-        -I/usr/local/cuda/include tests/csrc/fwi_host.cpp -o build/libfwi_asan.so
-    LD_PRELOAD=$(g++ -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 python tools/fwi_host_asan.py build/libfwi_asan.so
+    LD_PRELOAD=$(g++ -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 python tools/fwi_host_asan.py
 """
-import sys, os, ctypes
+import sys, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for d in (os.path.join(ROOT, "tests"), ROOT, os.path.join(ROOT, "tests", "golden")):
     sys.path.insert(0, d)
-if len(sys.argv) != 2:
-    raise SystemExit(__doc__)
 import numpy as np
 import fwi_host_build as hb
-hb._lib = ctypes.CDLL(os.path.abspath(sys.argv[1])); hb._lib.fwi_host_last_error.restype = ctypes.c_char_p
+import host_build
+hb.load = lambda: host_build.load("fwi_asan", "fwi_host.cpp", signatures=hb.SIGNATURES,
+                                  flags=("-O1", "-g", "-fsanitize=address,undefined", "-fno-omit-frame-pointer"))
 import make_golden as mg
 from test_fire_oracle import case_inputs, check_outputs
 g = np.load(os.path.join(ROOT, "tests", "golden", "ref_cffwis.npz"))

@@ -51,10 +51,15 @@ def sources() -> list[str]:
     return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cu"))
 
 
+def headers(*dirs: str) -> list[str]:
+    """Every header under csrc/ and include/ (and under ``dirs``): what any source may include."""
+    return sorted(os.path.join(d, f) for d in (CSRC, os.path.join(ROOT, "include"), *dirs)
+                  for f in os.listdir(d) if f.endswith((".cuh", ".h")))
+
+
 def _deps_mtime() -> float:
-    hdrs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
-    hdrs.append(os.path.join(ROOT, "include", "xclim_b200.h"))
-    return max(os.path.getmtime(h) for h in hdrs)
+    # this file too: a change of NVCC_FLAGS or EXTRA_FLAGS recompiles every object
+    return max(os.path.getmtime(h) for h in headers() + [os.path.abspath(__file__)])
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
