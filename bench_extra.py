@@ -557,6 +557,65 @@ def main():
                     "oracle_check": {"cells": int(cols.size), "max_rel_diff": rel(out[:, cols].cpu().numpy(), exp)},
                     **card})
         del tmax, out
+    if want("rainseason") and a.only:   # rain season: opt-in (--only rainseason), on the --lat band
+        import subprocess
+
+        from oracle import rain_season_oracle as RO
+        from xclim_b200 import TimeAxis
+        from xclim_b200.indices import _rain_season_mask
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True)
+        card = {"gpu": torch.cuda.get_device_name(), "power_limit": q.stdout.strip() or "unknown",
+                "frac_basis": "3.35 TB/s (H100 SXM data sheet)"}
+        del tas, pr
+        torch.cuda.empty_cache()
+        # daily pr in mm/d: a rainy season of 10-day regimes (4 in 5 wet, 3-15 mm a day; the others 0-2 mm) between
+        # a per-cell, per-year onset (doy 120-180) and cessation (doy 250-300), rare showers outside it, so that
+        # most cells find a start after 05-01 and an end in a 20-day dry spell after 09-01 under the defaults
+        g = torch.Generator(device="cuda").manual_seed(17)
+        x = torch.empty((T, C), dtype=torch.float32, device="cuda")
+        d = torch.arange(YEAR, device="cuda")[:, None]
+        for y in range(T // YEAR):
+            on = torch.randint(120, 181, (1, C), device="cuda", generator=g)
+            off = torch.randint(250, 301, (1, C), device="cuda", generator=g)
+            wet = (torch.rand((YEAR // 10 + 1, C), device="cuda", generator=g) < 0.8).repeat_interleave(10, 0)[:YEAR]
+            u = torch.rand((YEAR, C), device="cuda", generator=g)
+            season = (d >= on) & (d < off)
+            shower = torch.rand((YEAR, C), device="cuda", generator=g) < 0.02
+            x[y * YEAR:(y + 1) * YEAR] = torch.where(season, torch.where(wet, 3 + 12 * u, 2 * u),
+                                                     torch.where(shower, 5 * u, torch.zeros_like(u)))
+            del on, off, wet, u, season, shower
+        ta = TimeAxis.daily("1991-01-01", T, "noleap")
+        p = RO.DEFAULTS
+        mask = _rain_season_mask(ta, poff, p["date_min_start"], p["date_max_start"], p["date_min_end"],
+                                 p["date_max_end"])
+        s, e = device.rain_season(x, poff, mask, 1.0, p["thresh_wet_start"], p["window_wet_start"],
+                                  p["window_not_dry_start"], p["thresh_dry_start"], p["window_dry_start"],
+                                  0, p["thresh_dry_end"], p["window_dry_end"], 0)
+        # the kernel alone: the mask and the period offsets stay on the device between launches
+        lib = _lib.load()
+        mask_d = torch.from_numpy(mask).cuda()
+        poff_d = torch.from_numpy(poff).cuda()
+        st = torch.empty((P, C), dtype=torch.int32, device="cuda")
+        en = torch.empty_like(st)
+
+        def launch():
+            _lib.check(lib.xc_rain_season_f32(x.data_ptr(), T, C, C, poff_d.data_ptr(), P, mask_d.data_ptr(), 1.0,
+                                              25.0, 3, 30, 1.0, 7, 0, 0.0, 20, 0, st.data_ptr(), en.data_ptr(), None))
+        ms = timeit(launch, a.steps)
+        cols = np.unique(np.r_[np.linspace(0, C - 1, 96).astype(int), np.arange(C - 32, C)])
+        o = RO.rain_season(x[:, cols].cpu().numpy(), ta, "YS")
+        got_s = s[:, cols].cpu().numpy().astype(np.float64)
+        got_e = e[:, cols].cpu().numpy().astype(np.float64)
+        mism = int(np.sum(~np.isclose(np.where(got_s < 0, np.nan, got_s), o["start_idx"], equal_nan=True, rtol=0))
+                   + np.sum(~np.isclose(np.where(got_e < 0, np.nan, got_e), o["end_idx"], equal_nan=True, rtol=0)))
+        nb = T * C * 4 + 3 * P * C * 8
+        report(f"rain_season (defaults), {a.lat} x 1440 cells", ms, nb,
+               {"frac_of_3_35_tbs": nb / (ms * 1e-3) / 3.35e12,
+                "seasons_found": float((s >= 0).float().mean()), "ends_found": float((e >= 0).float().mean()),
+                "oracle_check": {"cells": int(cols.size), "mismatches": mism}, **card})
+        del x, s, e, st, en
+        torch.cuda.empty_cache()
     if want("fwi") and a.only:      # the fire-weather kernel: opt-in (--only fwi), never part of a default run
         import time
 

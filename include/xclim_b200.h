@@ -829,6 +829,31 @@ int32_t xc_pet_monthly_f32(const float* const* inputs, int64_t T, int64_t C, int
                            int64_t L, const int32_t* lat_index, const XcPetParams* params_host, float* out,
                            void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * r1  rain season (Sivakumar 1998) -- indices/_agro.py:790-980 `rain_season`, per period of freq.
+ *   x: (T, C) daily precipitation at x[t * ldx + c], ldx >= C, turned into amounts by one float32
+ *   multiply by `scale` (rate2amount to mm).  mask: device uint8 (T) shared by all cells:
+ *   XC_RS_PRE  inside the onset prefilter (date_min_start .. the last day of the step's period),
+ *   XC_RS_START inside [date_min_start, date_max_start], XC_RS_END inside [date_min_end, date_max_end];
+ *   every period must hold at least one step of each of the last two (the caller checks it).
+ *   Thresholds are in mm and compared in float32; methods are XC_RS_PER_DAY or XC_RS_TOTAL.
+ *   out_start, out_end: device int32 (P, C) at out[p * C + c], the step of the season's start and end
+ *   inside the period, -1 where there is none.  window_dry_start <= XC_RS_MAX_WINDOW, else
+ *   XC_ERR_UNSUPPORTED.  Semantics in xclim_b200/csrc/rain_season_core.cuh and DESIGN.md section 4.
+ * ------------------------------------------------------------------------------------------- */
+#define XC_RS_PER_DAY 0
+#define XC_RS_TOTAL   1
+#define XC_RS_PRE     1
+#define XC_RS_START   2
+#define XC_RS_END     4
+#define XC_RS_MAX_WINDOW 64
+int32_t xc_rain_season_f32(const float* x, int64_t T, int64_t C, int64_t ldx, const int32_t* period_offsets,
+                           int32_t P, const uint8_t* mask, float scale, double thresh_wet_start,
+                           int32_t window_wet_start, int32_t window_not_dry_start, double thresh_dry_start,
+                           int32_t window_dry_start, int32_t method_dry_start, double thresh_dry_end,
+                           int32_t window_dry_end, int32_t method_dry_end, int32_t* out_start, int32_t* out_end,
+                           void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -98,6 +98,8 @@ SIGNATURES = {
     "xc_ens_moments_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "xc_ens_robustness_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64,
                                      _vp, _i32, _f64, _i32, _vp, _vp, _vp]),
+    "xc_rain_season_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, C.c_float, _f64, _i32, _i32, _f64, _i32,
+                                  _i32, _f64, _i32, _i32, _vp, _vp, _vp]),
 }
 
 # ensembles (include/xclim_b200.h e1)
@@ -125,6 +127,12 @@ AN_STATUS_NOT_FINITE, AN_STATUS_CHKFINITE = 1, 2
 PET_METHODS = {"BR65": 0, "HG85": 1, "MB05": 2, "allen98": 3, "TW48": 4, "DA02": 5, "given": 6}
 PET_MONTHLY = ("TW48", "DA02")
 PET_INPUTS = ("tasmin", "tasmax", "tas", "hurs", "rsds", "rsus", "rlds", "rlus", "sfcWind", "pr", "evspsblpot")
+
+
+# rain season (include/xclim_b200.h r1)
+RS_METHODS = {"per_day": 0, "total": 1}
+RS_PRE, RS_START, RS_END = 1, 2, 4
+RS_MAX_WINDOW = 64
 
 
 class PetParams(C.Structure):

@@ -770,6 +770,28 @@ def pet_monthly(inputs, moff, yoff, mdays, table, lat_index, params):
     return out
 
 
+# ------------------------------------------------------------------------------------ rain season
+def rain_season(x2d, poff, mask, scale, thr_wet, window_wet, window_not_dry, thr_dry_start, window_dry_start,
+                method_dry_start, thr_dry_end, window_dry_end, method_dry_end):
+    """Steps of the rain season's start and end inside each period (xc_rain_season_f32): ``x2d`` (T, C) float32
+    device rates (a row stride > C works in place), ``mask`` (T,) uint8 host array of XC_RS_* bits, thresholds in
+    mm, methods ``_lib.RS_METHODS`` codes.  Returns two (P, C) int32 tensors, -1 where there is none."""
+    T, C = x2d.shape
+    assert C == 1 or x2d.stride(1) == 1      # a single column may carry any stride
+    dev = x2d.device
+    P = len(poff) - 1
+    poff_d = dev_ints(poff, np.int32, dev)
+    mask_d = torch.from_numpy(np.ascontiguousarray(mask, dtype=np.uint8)).to(dev)
+    start = torch.empty((P, C), dtype=torch.int32, device=dev)
+    end = torch.empty((P, C), dtype=torch.int32, device=dev)
+    check(load().xc_rain_season_f32(x2d.data_ptr(), T, C, x2d.stride(0), poff_d.data_ptr(), P, mask_d.data_ptr(),
+                                    float(scale), float(thr_wet), int(window_wet), int(window_not_dry),
+                                    float(thr_dry_start), int(window_dry_start), int(method_dry_start),
+                                    float(thr_dry_end), int(window_dry_end), int(method_dry_end), start.data_ptr(),
+                                    end.data_ptr(), current_stream_ptr()))
+    return start, end
+
+
 # ------------------------------------------------------------------------------------ ensembles
 def ens_percentiles(x2d, percentiles, alpha, beta, min_members):
     """Percentiles along the member axis of an (R, N) float32 matrix (xc_ens_percentiles_f32; column views with

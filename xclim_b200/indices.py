@@ -1162,6 +1162,93 @@ def _like(template, values, units):
                  template.name)
 
 
+# ------------------------------------------------------------------ agroclimatic detection indices (indices/_agro.py)
+def _month_day(value, name):
+    import re
+    m = re.fullmatch(r"(\d\d)-(\d\d)", value) if isinstance(value, str) else None
+    if m is None or not (1 <= int(m.group(1)) <= 12 and 1 <= int(m.group(2)) <= 31):
+        raise ValueError(f"{name} must be a 'MM-DD' string, got {value!r}")
+    return value
+
+
+def _rain_season_mask(ta, poff, date_min_start, date_max_start, date_min_end, date_max_end):
+    """uint8 (T,) of the steps ``select_time(date_bounds=...)`` keeps in each of the three selections of
+    `rain_season` (``_lib.RS_PRE | RS_START | RS_END``).  The onset prefilter ends on each period's own last day
+    (indices/_agro.py:905-906).  Raises ValueError where the start or the end bounds select no day of a period,
+    where the reference's ``nanargmax`` raises."""
+    import numpy as np
+
+    from . import _lib
+    mask = (_lib.RS_START * ta.select_mask(date_bounds=(date_min_start, date_max_start))
+            + _lib.RS_END * ta.select_mask(date_bounds=(date_min_end, date_max_end))).astype(np.uint8)
+    for p, (a, b) in enumerate(zip(poff[:-1], poff[1:])):
+        part = ta.isel(slice(int(a), int(b)))
+        last = f"{int(part.month[-1]):02d}-{int(part.day[-1]):02d}"
+        mask[a:b] |= (_lib.RS_PRE * part.select_mask(date_bounds=(date_min_start, last))).astype(np.uint8)
+        for bit, lo, hi in ((_lib.RS_START, date_min_start, date_max_start),
+                            (_lib.RS_END, date_min_end, date_max_end)):
+            if not (mask[a:b] & bit).any():
+                raise ValueError(f"date bounds ({lo}, {hi}) select no day of the period starting "
+                                 f"{ta.date_strings(int(a))[0]}")
+    return mask
+
+
+def rain_season(pr, thresh_wet_start="25.0 mm", window_wet_start=3, window_not_dry_start=30, thresh_dry_start="1.0 mm",
+                window_dry_start=7, method_dry_start="per_day", date_min_start="05-01", date_max_start="12-31",
+                thresh_dry_end="0.0 mm", window_dry_end=20, method_dry_end="per_day", date_min_end="09-01",
+                date_max_end="12-31", freq="YS-JAN"):
+    """Start and end (day of year) and length of the rain season -- indices/_agro.py:790-980 (Sivakumar 1998).
+
+    The season starts at the end of a wet spell (``thresh_wet_start`` accumulated over ``window_wet_start`` days)
+    that is followed by ``window_not_dry_start`` days with no dry sequence (``window_dry_start`` days at or below
+    ``thresh_dry_start``, each day or in total per ``method_dry_start``), between ``date_min_start`` and
+    ``date_max_start``.  It ends with the first dry sequence after the start (``thresh_dry_end``,
+    ``window_dry_end``, ``method_dry_end``) between ``date_min_end`` and ``date_max_end``.  Returns the float64
+    tuple ``(rain_season_start, rain_season_end, rain_season_length)``; the length runs to the period's end when no
+    end is found.  One kernel pass over ``pr`` per call (xc_rain_season_f32); window sums follow DESIGN.md
+    section 4, and ``window_dry_start`` is limited to 64 days (section 5)."""
+    import numpy as np
+    import torch
+
+    from . import _lib, device
+    from .generic import _unwrap, _wrap_periods
+    from .run_length import index_to_doy
+    from .units import convert_units_to, units_of
+    for name, m in (("method_dry_start", method_dry_start), ("method_dry_end", method_dry_end)):
+        if m not in _lib.RS_METHODS:
+            raise ValueError(f"Unknown {name}: {m}.")
+    windows = {"window_wet_start": window_wet_start, "window_not_dry_start": window_not_dry_start,
+               "window_dry_start": window_dry_start, "window_dry_end": window_dry_end}
+    for name, w in windows.items():
+        if not isinstance(w, (int, np.integer)) or w < (0 if name == "window_not_dry_start" else 1):
+            raise ValueError(f"{name} must be an integer >= {0 if name == 'window_not_dry_start' else 1}, got {w!r}")
+    if window_dry_start > _lib.RS_MAX_WINDOW:
+        raise NotImplementedError(f"window_dry_start above {_lib.RS_MAX_WINDOW} days is not supported")
+    dates = [_month_day(v, n) for v, n in ((date_min_start, "date_min_start"), (date_max_start, "date_max_start"),
+                                           (date_min_end, "date_min_end"), (date_max_end, "date_max_end"))]
+    scale = convert_units_to(f"1 {units_of(pr)}", "mm/d")           # rate2amount(pr, out_units="mm"), :892
+    thr = [convert_units_to(t, "mm") for t in (thresh_wet_start, thresh_dry_start, thresh_dry_end)]
+
+    x2d, cell_shape, other, ta = _unwrap(pr)
+    poff = ta.period_offsets(freq)
+    mask = _rain_season_mask(ta, poff, *dates)
+    start_i, end_i = device.rain_season(x2d, poff, mask, scale, thr[0], window_wet_start, window_not_dry_start, thr[1],
+                                        window_dry_start, _lib.RS_METHODS[method_dry_start], thr[2], window_dry_end,
+                                        _lib.RS_METHODS[method_dry_end])
+    nan = torch.tensor(float("nan"), dtype=torch.float64, device=start_i.device)
+    start = torch.where(start_i < 0, nan, start_i.to(torch.float64))
+    end = torch.where(end_i < 0, nan, end_i.to(torch.float64))
+    n = torch.from_numpy(np.diff(poff).astype(np.float64)).to(start.device)[:, None]
+    length = torch.where(end_i >= 0, end - start, n - start)
+    doy_attrs = {"units": "", "is_dayofyear": np.int32(1), "calendar": ta.calendar}
+    return (_wrap_periods(pr, index_to_doy(start, poff, ta), cell_shape, other, ta, freq, dict(doy_attrs),
+                          dtype=np.float64, name="rain_season_start"),
+            _wrap_periods(pr, index_to_doy(end, poff, ta), cell_shape, other, ta, freq, dict(doy_attrs),
+                          dtype=np.float64, name="rain_season_end"),
+            _wrap_periods(pr, length, cell_shape, other, ta, freq, {"units": "days"}, dtype=np.float64,
+                          name="rain_season_length"))
+
+
 # ---- end-to-end path: host-backed inputs stream through HBM in lat slabs (xclim_b200/streaming.py)
 def _stream_entry_points():
     import inspect
