@@ -18,6 +18,9 @@
 // that started earlier) and reads past the period end until its open runs close.  UNROLL
 // independent 16-byte loads are issued before any use so that each thread keeps >= 128 B in
 // flight; data is read exactly once (ld.global.nc.L1::no_allocate).
+#include <stdlib.h>
+
+#include <algorithm>
 #include <type_traits>
 
 #include "runstat.cuh"
@@ -125,6 +128,72 @@ period_runstat_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t
   }
   store_vec<VEC>(out + (int64_t)p * C + c0, res);
   if constexpr (VALID) store_vec<VEC>(valid + (int64_t)p * C + c0, nv);
+}
+
+// The same statistic for a scalar threshold with runs cut at the period edges (AFTER == false), fed by the bulk-copy
+// row ring (BulkRows, runstat.cuh): a persistent grid walks the (period, tile of kBulkCells cells) work items
+// period-major, so that the CTAs running together stream the same rows and the tail is one item, not a partial wave.
+// Every element goes through the same cmp / valid increment / run_step, in time order, as in period_runstat_kernel:
+// the results are identical.
+constexpr int kBulkCells = 4096;
+constexpr int kBulkGroups = 4;   // 4-cell groups per consumer thread: 16 cells, 256 consumers
+using RunRing = BulkRows<kBulkCells, 4, 3, kBulkGroups>;
+constexpr int kBulkThreads = RunRing::kConsumers + 32;   // + one producer warp
+
+template <int OP, int RED, bool VALID, bool FASTMAX>
+__global__ void __launch_bounds__(kBulkThreads, 1)
+period_runstat_bulk_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, const int32_t* __restrict__ poff,
+                           int32_t P, float thr, int32_t window, float* __restrict__ out, int32_t* __restrict__ valid) {
+  constexpr int N = 4 * kBulkGroups;
+  extern __shared__ __align__(128) unsigned char smem[];
+  RunRing ring;
+  ring.init(smem);
+  const int64_t ntiles = (C + kBulkCells - 1) / kBulkCells;
+  const int64_t items = ntiles * P;
+  if (threadIdx.x >= RunRing::kConsumers) {
+    if (threadIdx.x == RunRing::kConsumers) {
+      for (int64_t it = blockIdx.x; it < items; it += gridDim.x) {
+        const int p = (int)(it / ntiles);
+        const int64_t c0 = (it - (int64_t)p * ntiles) * kBulkCells;
+        ring.produce(x + c0, ldx, (int)min((int64_t)kBulkCells, C - c0), __ldg(poff + p), __ldg(poff + p + 1));
+      }
+    }
+    return;
+  }
+  const int j = threadIdx.x;
+  for (int64_t it = blockIdx.x; it < items; it += gridDim.x) {
+    const int p = (int)(it / ntiles);
+    const int64_t c0 = (it - (int64_t)p * ntiles) * kBulkCells;
+    int32_t cur[N], nv[N];
+    RunAcc<RED> acc[N];
+#pragma unroll
+    for (int i = 0; i < N; ++i) { cur[i] = 0; nv[i] = 0; acc[i].init(); }
+    ring.consume(j, __ldg(poff + p), __ldg(poff + p + 1), [&](int v, const Vec<4>& r) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int i = 4 * v + e;
+        const bool m = cmp<OP>(r.v[e], thr);
+        if constexpr (VALID) nv[i] += (r.v[e] == r.v[e]) ? 1 : 0;
+        run_step<FASTMAX>(cur[i], acc[i], m, window);
+      }
+    });
+#pragma unroll
+    for (int v = 0; v < kBulkGroups; ++v) {
+      const int64_t c = c0 + 4 * (j + v * RunRing::kConsumers);
+      if (c < C) {
+        float res[4];
+        int32_t n[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          run_close<FASTMAX>(cur[4 * v + e], acc[4 * v + e], window);
+          res[e] = acc[4 * v + e].result();
+          n[e] = nv[4 * v + e];
+        }
+        store_vec<4>(out + (int64_t)p * C + c, res);
+        if constexpr (VALID) store_vec<4>(valid + (int64_t)p * C + c, n);
+      }
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -601,12 +670,36 @@ extern "C" int32_t xc_period_count_f32(const float* x, int64_t T, int64_t C, int
 }
 
 namespace {
-// v4: the layout of the threshold source allows 4 cells per thread as well
+template <int OP, int RED, bool FASTMAX, bool VALID>
+int32_t launch_runstat_bulk(const float* x, int64_t C, int64_t ldx, const int32_t* poff, int32_t P, float thr,
+                            int32_t window, float* out, int32_t* valid, cudaStream_t st) {
+  auto* kernel = period_runstat_bulk_kernel<OP, RED, VALID, FASTMAX>;
+  constexpr size_t smem = RunRing::kSmemBytes;
+  if (int32_t e = allow_smem(kernel, smem, "period_runstat_bulk_kernel")) return e;
+  int per_sm = 0;
+  XC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kBulkThreads, smem));
+  const int64_t items = (C + kBulkCells - 1) / kBulkCells * P;
+  const int grid = (int)std::min<int64_t>(items, (int64_t)sm_count() * std::max(per_sm, 1));
+  kernel<<<grid, kBulkThreads, smem, st>>>(x, C, ldx, poff, P, thr, window, out, valid);
+  return launch_status("period_runstat_bulk_kernel");
+}
+
+// v4: the layout of the threshold source allows 4 cells per thread as well.  A scalar threshold with runs cut at
+// the period edges on at least one tile of cells goes to the bulk-copy kernel, unless XCLIM_B200_RUNSTAT_V1 is set
+// (the per-lane kernel for every call: the two give identical results, and tests compare them).  The std reducer
+// stays on the per-lane kernel.
 template <int OP, int RED, bool FASTMAX, typename THR>
 int32_t launch_runstat(const float* x, int64_t T, int64_t C, int64_t ldx, const int32_t* poff, int32_t P,
                        THR thr, int32_t window, bool after, float* out, int32_t* valid, cudaStream_t st,
                        bool thr_v4 = true) {
   const bool v4 = can_vec4(x, C, ldx, out, valid) && thr_v4;
+  // std keeps the per-lane kernel: its 64-bit sums of squares for 16 cells per thread spill in the bulk kernel
+  if constexpr (std::is_same_v<THR, ScalarThr> && RED != XC_RL_STD) {
+    if (v4 && !after && C >= kBulkCells && !getenv("XCLIM_B200_RUNSTAT_V1")) {
+      return valid ? launch_runstat_bulk<OP, RED, FASTMAX, true>(x, C, ldx, poff, P, thr.t, window, out, valid, st)
+                   : launch_runstat_bulk<OP, RED, FASTMAX, false>(x, C, ldx, poff, P, thr.t, window, out, valid, st);
+    }
+  }
   auto go = [&](auto VECC, auto VALC, auto AFTC) -> int32_t {
     constexpr int VEC = decltype(VECC)::value;
     constexpr bool VAL = decltype(VALC)::value;
