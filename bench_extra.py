@@ -128,6 +128,17 @@ def main():
                                                  _lib.RL_REDUCERS["max"]), a.steps)
         report("spell_runstat window=5 min>291.15 max (spell_runstat4_kernel)", ms, T * C * 4 + P * C * 4,
                cpu=lambda: O.spell_length_statistics(host["tas"], 291.15, 5, "min", ">", "max", poff))
+    if want("spell10"):   # a window past the register kernels' 2..8: the ring's sliding float64 sum
+        ms = timeit(lambda: device.spell_runstat(pr, poff, 10, _lib.STATS["sum"], _lib.OPS["<"], 1.0,
+                                                 _lib.RL_REDUCERS["count"]), a.steps)
+        report("spell_runstat window=10 sum<1 count (spell_runstat4_kernel, sliding sum)", ms, T * C * 4 + P * C * 4,
+               cpu=lambda: O.spell_length_statistics(host["pr"], 1.0, 10, "sum", "<", "count", poff))
+    if want("rolling1"):
+        ms = timeit(lambda: device.rolling_period_reduce(pr, poff, 1, _lib.STATS["sum"], False, _lib.STATS["min"]),
+                    a.steps)
+        report("rolling(1).sum -> min (rolling_period_reduce4_kernel, sliding sum)", ms, T * C * 4 + P * C * 4,
+               cpu=lambda: O.select_rolling_resample_op(host["pr"], "min", 1, poff, window_center=False,
+                                                        window_op="sum"))
     if want("gap"):
         ms = timeit(lambda: device.period_runstat_gap(pr, poff, _lib.OPS["<"], 1.0, _lib.RL_REDUCERS["max"], 3),
                     a.steps)

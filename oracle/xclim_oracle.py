@@ -661,6 +661,88 @@ def select_rolling_resample_op(x, op, window, poff, window_center=True, window_o
     return resample_reduce(rolling(x, window, window_op, center=window_center), poff, op)
 
 
+def window_stat_rule(x, window, stat):
+    """The kernels' window statistic (DESIGN §4, ``window_stat`` in csrc/rolling.cu), right-aligned: the value
+    at t covers x[t-window+1 .. t] (NaN for t < window-1).  A sum is the float64 sum of the window's values
+    from the oldest to the newest, one add at a time (np.sum would pair them up), rounded once to float32; a
+    mean is (float)(sum / window); min and max are taken in float32.  A window holding a NaN is NaN."""
+    x = np.asarray(x, dtype=np.float32)
+    out = np.full(x.shape, np.nan, dtype=np.float32)
+    n = x.shape[0] - window + 1
+    if n <= 0:
+        return out
+    with np.errstate(all="ignore"):
+        if stat in ("sum", "mean"):
+            s = np.zeros((n,) + x.shape[1:], dtype=np.float64)
+            for k in range(window):
+                s = s + x[k:k + n].astype(np.float64)
+            out[window - 1:] = (s / window if stat == "mean" else s).astype(np.float32)
+        else:
+            fn = np.fmin if stat == "min" else np.fmax
+            m = x[:n].copy()
+            nan = np.isnan(m)
+            for k in range(1, window):
+                m = fn(m, x[k:k + n])
+                nan |= np.isnan(x[k:k + n])
+            out[window - 1:] = np.where(nan, np.float32(np.nan), m)
+    return out
+
+
+def spell_mask_rule(x, window, stat, op, thresh):
+    """The kernels' spell mask: step t is in a spell if some length-``window`` block that lies fully inside the
+    series and contains t has (window statistic op float32(thresh)); a NaN window only satisfies ``!=``.
+    The reference pads the series end with NaN instead (spell_mask above), which differs under ``!=`` only."""
+    x = np.asarray(x, dtype=np.float32)
+    T = x.shape[0]
+    cond = np.zeros(x.shape, dtype=bool)           # cond[i]: block [i, i+window-1]
+    with np.errstate(invalid="ignore"):
+        cond[:T - window + 1] = compare(window_stat_rule(x, window, stat)[window - 1:], op, np.float32(thresh))
+    mask = cond.copy()
+    for k in range(1, window):
+        mask[k:] |= cond[:T - k]
+    return mask
+
+
+def rolling_rule(x, window, stat, center=False):
+    """``rolling(time=window, center=center).<stat>()`` under the kernels' window rule: the value labelled t
+    covers the window ending at t + shift (shift = window // 2 when centred); incomplete windows are NaN."""
+    r = window_stat_rule(x, window, stat)
+    return _shift(r, -(window // 2), np.nan) if center else r
+
+
+def period_stat_rule(vals, poff, stat):
+    """Per-period statistic of float32 values as the kernels' StatAcc takes it: NaN skipped, sum and sum of
+    squares in float64 in time order, rounded once; var = E[v^2] - E[v]^2 clamped at 0 (one pass)."""
+    vals = np.asarray(vals, dtype=np.float32)
+    out = []
+    with np.errstate(all="ignore"), _quiet():
+        for s0, e0 in _groups(poff):
+            blk = vals[s0:e0]
+            ok = ~np.isnan(blk)
+            n = ok.sum(axis=0)
+            s = np.zeros(blk.shape[1:], dtype=np.float64)
+            q = np.zeros(blk.shape[1:], dtype=np.float64)
+            for v, k in zip(blk.astype(np.float64), ok):
+                s = s + np.where(k, v, 0.0)
+                q = q + np.where(k, v * v, 0.0)
+            if stat == "sum":
+                r = s
+            elif stat == "count":
+                r = n.astype(np.float64)
+            elif stat == "mean":
+                r = np.where(n > 0, s / n, np.nan)
+            elif stat in ("min", "max"):
+                r = getattr(np, "nan" + stat)(np.where(ok, blk, np.nan), axis=0) if blk.shape[0] else \
+                    np.full(blk.shape[1:], np.nan)
+            else:
+                mean = s / n
+                var = q / n - mean * mean
+                var = np.where(var > 0.0, var, 0.0)
+                r = np.where(n > 0, np.sqrt(var) if stat == "std" else var, np.nan)
+            out.append(np.asarray(r).astype(np.float32))
+    return np.stack(out, axis=0)
+
+
 def tg_mean(tas, poff):
     """indices/_simple.py:113."""
     return select_resample_op(tas, "mean", poff)

@@ -55,21 +55,48 @@ __device__ __forceinline__ float window_stat(const float* __restrict__ col, int6
   }
 }
 
-// Sliding window state for sum / mean windows: running float64 sum of the non-NaN values plus the
-// number of NaNs in the window.  Sums of float32 values whose exponents lie within a few decades of
-// each other are exact in float64, so the running sum equals the direct sum of the w values.
+// s += v; true when the float64 add is exact.  r = s + v exactly <=> r - s == v and r - v == s (the
+// difference with the larger operand is computed exactly, Fast2Sum), and an infinity fails the test (inf - inf).
+__device__ __forceinline__ bool add_exact(double& s, double v) {
+  const double r = s + v;
+  const bool ok = (r - s == v) & (r - v == s);
+  s = r;
+  return ok;
+}
+
+// Sliding window state for sum / mean windows: float64 sum of the non-NaN values plus the number of NaNs in
+// the window.  A running sum (new value in, oldest out) is the window_stat value only while it is exact: an
+// infinity leaving the window would leave NaN behind (inf - inf), and a value that absorbed its neighbours
+// (the 9.97e36 netCDF fill) would leave their loss behind.  So every update is checked, and a window reached
+// through a rounded update is summed again directly, oldest value first -- exactly window_stat's sum.  That
+// happens only while the window holds such a value: on ordinary data every update is exact.
 struct SlideSum {
   double s;
   int nan;
-  __device__ __forceinline__ void add(float v) {
-    const bool bad = (v != v);
-    nan += bad ? 1 : 0;
-    s += bad ? 0.0 : (double)v;
+  bool exact;     // s is the exact sum of the window's non-NaN values
+  // the direct sum of x[i .. i+w-1]
+  __device__ __forceinline__ void load(const float* __restrict__ col, int64_t ldx, int i, int w) {
+    s = 0.0;
+    nan = 0;
+    exact = true;
+    for (int k = 0; k < w; ++k) {
+      const float v = __ldg(col + (int64_t)(i + k) * ldx);
+      if (v != v) ++nan;
+      else exact &= add_exact(s, (double)v);
+    }
   }
-  __device__ __forceinline__ void drop(float v) {
-    const bool bad = (v != v);
-    nan -= bad ? 1 : 0;
-    s -= bad ? 0.0 : (double)v;
+  // window [i, i+w-1] -> [i+1, i+w]: vin = x[i+w] enters, vout = x[i] leaves
+  __device__ __forceinline__ void slide(float vin, float vout, const float* __restrict__ col, int64_t ldx, int i,
+                                        int w) {
+    bool ok = exact;
+    if (vin != vin) ++nan;
+    else ok &= add_exact(s, (double)vin);
+    if (vout != vout) --nan;
+    else ok &= add_exact(s, -(double)vout);
+    if (!ok) load(col, ldx, i + 1, w);
+  }
+  __device__ __forceinline__ float value(int wstat, int w) const {
+    return nan ? NAN : (float)(wstat == XC_STAT_MEAN ? s / (double)w : s);
   }
 };
 
@@ -88,16 +115,14 @@ rolling_period_reduce_kernel(const float* __restrict__ x, int64_t T, int64_t C, 
   acc.init(stat);
   // the value labelled t covers x[i .. i+w-1], i = t + shift - w + 1 (shift 0: right-aligned, w/2: centred)
   if (wstat == XC_STAT_SUM || wstat == XC_STAT_MEAN) {
-    const double inv = (wstat == XC_STAT_MEAN) ? 1.0 / (double)w : 1.0;
     int t = t0;
     // labels whose window is incomplete at the series start give NaN
     while (t < t1 && t + shift - w + 1 < 0) ++t;
-    SlideSum win{0.0, 0};
+    SlideSum win;
     int i = t + shift - w + 1;          // first complete window of this period
-    if (t < t1 && i + w <= (int)T)
-      for (int k = 0; k < w; ++k) win.add(__ldg(col + (int64_t)(i + k) * ldx));
+    if (t < t1 && i + w <= (int)T) win.load(col, ldx, i, w);
     while (t < t1 && i + w <= (int)T) {
-      acc.take(win.nan ? NAN : (float)(wstat == XC_STAT_MEAN ? win.s / (double)w : win.s));
+      acc.take(win.value(wstat, w));
       // slide by up to kChunk steps with all loads issued first
       const int steps = min(kChunk, min(t1 - 1 - t, (int)T - (i + w)));
       if (steps <= 0) break;
@@ -112,15 +137,13 @@ rolling_period_reduce_kernel(const float* __restrict__ x, int64_t T, int64_t C, 
 #pragma unroll
       for (int k = 0; k < kChunk; ++k) {
         if (k < steps) {
-          win.add(vin[k]);
-          win.drop(vout[k]);
-          if (k + 1 < steps) acc.take(win.nan ? NAN : (float)(wstat == XC_STAT_MEAN ? win.s / (double)w : win.s));
+          win.slide(vin[k], vout[k], col, ldx, i + k, w);
+          if (k + 1 < steps) acc.take(win.value(wstat, w));
         }
       }
       t += steps;
       i += steps;
     }
-    (void)inv;
   } else {
     for (int t = t0; t < t1; ++t) {
       const int i = t + shift - w + 1;
@@ -137,7 +160,7 @@ rolling_period_reduce_kernel(const float* __restrict__ x, int64_t T, int64_t C, 
 // the mask per period (window == 1 on the mask, generic.py:562-570).
 //
 // The block statistics are produced in time order by BlockStream: for sum / mean windows a sliding
-// float64 sum (+ NaN counter), two loads per step; for min / max windows the w values are re-read
+// float64 sum (+ NaN counter, SlideSum), two loads per step; for min / max windows the w values are re-read
 // (L1 hits).
 struct BlockStream {
   const float* col;
@@ -151,8 +174,6 @@ struct BlockStream {
   __device__ __forceinline__ void init(int start) {
     i = start;
     primed = false;
-    win.s = 0.0;
-    win.nan = 0;
   }
   // short windows are cheaper to re-read (L1 hits) than to slide with float64 adds
   __device__ __forceinline__ bool sliding() const { return (wstat == XC_STAT_SUM || wstat == XC_STAT_MEAN) && w > 6; }
@@ -161,14 +182,12 @@ struct BlockStream {
     float r;
     if (sliding()) {
       if (!primed) {
-        for (int k = 0; k < w; ++k) win.add(__ldg(col + (int64_t)(i + k) * ldx));
+        win.load(col, ldx, i, w);
         primed = true;
       }
-      r = win.nan ? NAN : (float)(wstat == XC_STAT_MEAN ? win.s / (double)w : win.s);
-      if (i + 1 + w <= T) {  // slide to i + 1: one new row, one row re-read from L1/L2
-        win.add(__ldg(col + (int64_t)(i + w) * ldx));
-        win.drop(__ldg(col + (int64_t)i * ldx));
-      }
+      r = win.value(wstat, w);
+      if (i + 1 + w <= T)    // slide to i + 1: one new row, one row re-read from L1/L2
+        win.slide(__ldg(col + (int64_t)(i + w) * ldx), __ldg(col + (int64_t)i * ldx), col, ldx, i, w);
     } else {
       r = window_stat(col, ldx, i, w, wstat);
     }
@@ -218,28 +237,55 @@ spell_runstat_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t 
 // Streaming variants: a thread owns 4 adjacent cells (128-bit loads), walks the rows of one period
 // once and keeps the last w rows of its cells in a shared-memory ring [w][kThreads] of float4 (each
 // thread only touches its own column: no synchronisation).  Sum / mean windows slide a float64 sum
-// (new row in, ring row out); min / max windows rescan the ring.  DRAM traffic is one read of the
-// input (+ w-1 halo rows per period) and nothing is re-read through L1/L2, so these run at the
+// (new row in, ring row out; SlideSum's rule: re-summed from the ring after a rounded update); min / max
+// windows rescan the ring.  DRAM traffic is one read of the input (+ w-1 halo rows per period) and
+// nothing is re-read through L1/L2, so these run at the
 // speed of the window == 1 kernels instead of the latency-bound lane-per-cell kernels above, which
 // remain as the fall-back for unaligned inputs and windows that do not fit shared memory.
 // ------------------------------------------------------------------------------------------------
 constexpr int kU = 4;  // rows in flight per thread
 
+// SlideSum for the 4 cells of a thread; a window reached through a rounded update is summed again from the ring
 struct Win4 {
   double s[4];
   int nan[4];
+  bool exact[4];
   __device__ __forceinline__ void clear() {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) { s[j] = 0.0; nan[j] = 0; }
+    for (int j = 0; j < 4; ++j) { s[j] = 0.0; nan[j] = 0; exact[j] = true; }
   }
-  __device__ __forceinline__ void slide(const float4& vin, const float4& vout) {
+  // appends a row: while priming, s is the direct sum of the rows appended so far
+  __device__ __forceinline__ void push(const float4& v) {
+    const float a[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (a[j] != a[j]) ++nan[j];
+      else exact[j] &= add_exact(s[j], (double)a[j]);
+    }
+  }
+  // vin entered and vout left; the ring holds the new window, its oldest row at `slot`
+  __device__ __forceinline__ void slide(const float4& vin, const float4& vout, const float4* __restrict__ ring,
+                                        int lane, int w, int slot) {
     const float a[4] = {vin.x, vin.y, vin.z, vin.w};
     const float b[4] = {vout.x, vout.y, vout.z, vout.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const bool ba = (a[j] != a[j]), bb = (b[j] != b[j]);
-      nan[j] += (ba ? 1 : 0) - (bb ? 1 : 0);
-      s[j] += (ba ? 0.0 : (double)a[j]) - (bb ? 0.0 : (double)b[j]);
+      bool ok = exact[j];
+      if (a[j] != a[j]) ++nan[j];
+      else ok &= add_exact(s[j], (double)a[j]);
+      if (b[j] != b[j]) --nan[j];
+      else ok &= add_exact(s[j], -(double)b[j]);
+      if (!ok) {
+        s[j] = 0.0;
+        nan[j] = 0;
+        exact[j] = true;
+        for (int k = 0, r = slot; k < w; ++k, r = (r + 1 == w) ? 0 : r + 1) {
+          const float4 v = ring[r * kThreads + lane];
+          const float c[4] = {v.x, v.y, v.z, v.w};
+          if (c[j] != c[j]) ++nan[j];
+          else exact[j] &= add_exact(s[j], (double)c[j]);
+        }
+      }
     }
   }
 };
@@ -283,7 +329,7 @@ __device__ __forceinline__ void prime_ring(const float* __restrict__ col, int64_
     for (int k = 0; k < kU; ++k) {
       if (r + k < r1) {
         ring[slot * kThreads + lane] = v[k];
-        win.slide(v[k], zero);
+        win.push(v[k]);
         slot = (slot + 1 == w) ? 0 : slot + 1;
       }
     }
@@ -323,7 +369,7 @@ rolling_period_reduce4_kernel(const float* __restrict__ x, int64_t T, int64_t C,
         const float4 old = ring4[slot * kThreads + lane];
         ring4[slot * kThreads + lane] = v[k];
         slot = (slot + 1 == w) ? 0 : slot + 1;
-        win.slide(v[k], old);
+        if (wstat == XC_STAT_SUM || wstat == XC_STAT_MEAN) win.slide(v[k], old, ring4, lane, w, slot);
         float r[4];
         window_stat4(win, ring4, lane, w, wstat, r);
 #pragma unroll
@@ -385,7 +431,7 @@ spell_runstat4_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t
         const float4 old = ring4[slot * kThreads + lane];
         ring4[slot * kThreads + lane] = v[k];
         slot = (slot + 1 == w) ? 0 : slot + 1;
-        win.slide(v[k], old);
+        if (wstat == XC_STAT_SUM || wstat == XC_STAT_MEAN) win.slide(v[k], old, ring4, lane, w, slot);
         float r[4];
         window_stat4(win, ring4, lane, w, wstat, r);
         const int e = s + k, t = e - w + 1;
