@@ -712,35 +712,10 @@ def rolling_rule(x, window, stat, center=False):
 
 def period_stat_rule(vals, poff, stat):
     """Per-period statistic of float32 values as the kernels' StatAcc takes it: NaN skipped, sum and sum of
-    squares in float64 in time order, rounded once; var = E[v^2] - E[v]^2 clamped at 0 (one pass)."""
-    vals = np.asarray(vals, dtype=np.float32)
-    out = []
-    with np.errstate(all="ignore"), _quiet():
-        for s0, e0 in _groups(poff):
-            blk = vals[s0:e0]
-            ok = ~np.isnan(blk)
-            n = ok.sum(axis=0)
-            s = np.zeros(blk.shape[1:], dtype=np.float64)
-            q = np.zeros(blk.shape[1:], dtype=np.float64)
-            for v, k in zip(blk.astype(np.float64), ok):
-                s = s + np.where(k, v, 0.0)
-                q = q + np.where(k, v * v, 0.0)
-            if stat == "sum":
-                r = s
-            elif stat == "count":
-                r = n.astype(np.float64)
-            elif stat == "mean":
-                r = np.where(n > 0, s / n, np.nan)
-            elif stat in ("min", "max"):
-                r = getattr(np, "nan" + stat)(np.where(ok, blk, np.nan), axis=0) if blk.shape[0] else \
-                    np.full(blk.shape[1:], np.nan)
-            else:
-                mean = s / n
-                var = q / n - mean * mean
-                var = np.where(var > 0.0, var, 0.0)
-                r = np.where(n > 0, np.sqrt(var) if stat == "std" else var, np.nan)
-            out.append(np.asarray(r).astype(np.float32))
-    return np.stack(out, axis=0)
+    squares in float64 in time order, rounded once; var = E[v^2] - E[v]^2 clamped at 0 (one pass).  The rule
+    itself is oracle/stat_rule.py's period_stat."""
+    from oracle import stat_rule
+    return stat_rule.period_stat(vals, poff, stat)
 
 
 def tg_mean(tas, poff):

@@ -321,14 +321,15 @@ period_reduce_kernel(const float* __restrict__ x, int64_t C, int64_t ldx,
     if constexpr (STAT == XC_STAT_MEAN) res[i] = n[i] ? (float)(s[i] / nn) : NAN;
     if constexpr (STAT == XC_STAT_MIN || STAT == XC_STAT_MAX) res[i] = n[i] ? m[i] : NAN;
     if constexpr (STAT == XC_STAT_STD || STAT == XC_STAT_VAR) {
-      // stat_result()'s formula, kept as a copy: calling it reorders the register allocation of this kernel
+      // stat_result()'s formula, kept as a copy: calling it reorders the register allocation of this kernel.
+      // Every operation rounded, as there: this file is built with -fmad.
       if (n[i] == 0) {
         res[i] = NAN;
       } else {
-        double mean = s[i] / nn;
-        double var = q[i] / nn - mean * mean;
+        const double mean = __ddiv_rn(s[i], nn);
+        double var = __dsub_rn(__ddiv_rn(q[i], nn), __dmul_rn(mean, mean));
         var = var > 0.0 ? var : 0.0;
-        res[i] = (STAT == XC_STAT_STD) ? (float)sqrt(var) : (float)var;
+        res[i] = (STAT == XC_STAT_STD) ? (float)__dsqrt_rn(var) : (float)var;
       }
     }
   }

@@ -680,7 +680,8 @@ rolling_sumw_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t l
   float res[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    // stat_result()'s formula, kept as a copy: calling it changes this kernel's code
+    // stat_result()'s formula, kept as a copy: calling it changes this kernel's code.  Every operation rounded, as
+    // there: this file is built with -fmad.
     const double nn = (double)n[j];
     switch (stat) {
       case XC_STAT_SUM: res[j] = (float)s[j]; break;
@@ -690,10 +691,10 @@ rolling_sumw_kernel(const float* __restrict__ x, int64_t T, int64_t C, int64_t l
       case XC_STAT_MAX: res[j] = n[j] ? (float)(is_mean ? m[j] / (double)W : m[j]) : NAN; break;
       default: {
         if (!n[j]) { res[j] = NAN; break; }
-        const double mean = s[j] / nn;
-        double var = q[j] / nn - mean * mean;
+        const double mean = __ddiv_rn(s[j], nn);
+        double var = __dsub_rn(__ddiv_rn(q[j], nn), __dmul_rn(mean, mean));
         var = var > 0.0 ? var : 0.0;
-        res[j] = (stat == XC_STAT_STD) ? (float)sqrt(var) : (float)var;
+        res[j] = (stat == XC_STAT_STD) ? (float)__dsqrt_rn(var) : (float)var;
       }
     }
   }

@@ -259,15 +259,23 @@ __device__ __forceinline__ void stream_rows_thr(const float* __restrict__ col, i
 // Reducer value of a RunAcc that keeps every quantity and picks the reducer at run time (result(int)).
 constexpr int kRunAny = -1;
 
-// mean and std of n run lengths with sum s and sum of squares q; 0 when there is no run
+// mean and std of n run lengths with sum s and sum of squares q; 0 when there is no run.  The variance is
+// stat_result()'s, every operation rounded on the device (no contraction into a fused multiply-add).
 XC_RS_HD float run_mean(int32_t n, int32_t s) {
   return n == 0 ? 0.f : (float)((double)s / (double)n);
 }
 XC_RS_HD float run_std(int32_t n, int32_t s, unsigned long long q) {
   if (n == 0) return 0.f;
-  double nn = (double)n, m = (double)s / nn;
-  double var = (double)q / nn - m * m;
+  const double nn = (double)n;
+#ifdef __CUDA_ARCH__
+  const double m = __ddiv_rn((double)s, nn);
+  const double var = __dsub_rn(__ddiv_rn((double)q, nn), __dmul_rn(m, m));
+  return (float)__dsqrt_rn(var > 0.0 ? var : 0.0);
+#else
+  const double m = (double)s / nn;
+  const double var = (double)q / nn - m * m;
   return (float)sqrt(var > 0.0 ? var : 0.0);
+#endif
 }
 
 // Per-cell accumulator over the run lengths L >= window attributed to the period.
@@ -380,7 +388,10 @@ struct PeriodMask {
 };
 
 // Statistic of n non-NaN values with float64 sum s and sum of squares q and their min or max m.  Mean, min and
-// max of no values are NaN; std and var are q/n - mean^2 clamped at 0.
+// max of no values are NaN; std and var are q/n - mean^2 clamped at 0, each operation rounded to float64 with the
+// _rn intrinsics: a fused multiply-add (-fmad) would round mean^2 differently, and the difference cancels to
+// exactly what low-variance cells (a constant cell's 0) are made of.  oracle/stat_rule.py restates the rule that
+// tests/test_gpu_stat_rule.py holds every copy of it to, bit for bit.
 __device__ __forceinline__ float stat_result(int stat, int32_t n, double s, double q, float m) {
   const double nn = (double)n;
   switch (stat) {
@@ -391,10 +402,10 @@ __device__ __forceinline__ float stat_result(int stat, int32_t n, double s, doub
     case XC_STAT_MAX: return n ? m : NAN;
     default: {
       if (!n) return NAN;
-      const double mean = s / nn;
-      double var = q / nn - mean * mean;
+      const double mean = __ddiv_rn(s, nn);
+      double var = __dsub_rn(__ddiv_rn(q, nn), __dmul_rn(mean, mean));
       var = var > 0.0 ? var : 0.0;
-      return (stat == XC_STAT_STD) ? (float)sqrt(var) : (float)var;
+      return (stat == XC_STAT_STD) ? (float)__dsqrt_rn(var) : (float)var;
     }
   }
 }
