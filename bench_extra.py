@@ -627,6 +627,66 @@ def main():
                 "oracle_check": {"cells": int(cols.size), "mismatches": mism}, **card})
         del x, s, e, st, en
         torch.cuda.empty_cache()
+    if want("chill") and a.only:   # chill portions and units: opt-in (--only chill), fused from daily tasmin/tasmax
+        import subprocess
+
+        from oracle import chill_oracle as CO
+        from xclim_b200 import TimeAxis, converters
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True)
+        card = {"gpu": torch.cuda.get_device_name(), "power_limit": q.stdout.strip() or "unknown"}
+        del tas, pr
+        torch.cuda.empty_cache()
+        # daily tasmin / tasmax in degC over the band's latitudes (-89.75 .. -45.25 for 180 rows of a 0.25 grid):
+        # a seasonal cycle of the cell's hemisphere plus noise, tasmax 2-14 degC above tasmin
+        g = torch.Generator(device="cuda").manual_seed(23)
+        ta = TimeAxis.daily("1991-01-01", T, "noleap")
+        lats = -89.875 + 0.25 * np.arange(a.lat)
+        season = torch.from_numpy(np.cos(2 * np.pi * (ta.doy - 15) / 365.0).astype(np.float32)).cuda()[:, None]
+        lo = 2.0 + 8.0 * season + 4.0 * torch.randn((T, C), device="cuda", generator=g)
+        hi = lo + 2.0 + 12.0 * torch.rand((T, C), device="cuda", generator=g)
+        idx_np = np.repeat(np.arange(a.lat, dtype=np.int32), X)
+        w = torch.from_numpy(converters.hourly_weights(ta, lats)).cuda()
+        idx = torch.from_numpy(idx_np).cuda()
+        poff_j = ta.period_offsets("YS-JUL")
+        mask = ta.select_mask(date_bounds=("09-01", "03-30"))
+        Pj = poff_j.size - 1
+        lib = _lib.load()
+        poff_d = torch.from_numpy(poff_j).cuda()
+        mask_d = torch.from_numpy(mask.astype(np.uint8)).cuda()
+        cp = torch.empty((Pj, C), dtype=torch.float64, device="cuda")
+        cu = torch.empty((P, C), dtype=torch.float64, device="cuda")
+        poff_y = torch.from_numpy(poff).cuda()
+
+        def launch_cp():
+            _lib.check(lib.xc_chill_daily_f32(lo.data_ptr(), hi.data_ptr(), T, C, C, w.data_ptr(), a.lat,
+                                              idx.data_ptr(), poff_d.data_ptr(), Pj, mask_d.data_ptr(), 1.0, 273.15,
+                                              1.0, 0.0, _lib.CHILL_PORTIONS, cp.data_ptr(), None, None, None))
+
+        def launch_cu():
+            _lib.check(lib.xc_chill_daily_f32(lo.data_ptr(), hi.data_ptr(), T, C, C, w.data_ptr(), a.lat,
+                                              idx.data_ptr(), poff_y.data_ptr(), P, None, 1.0, 273.15, 1.0, 0.0,
+                                              _lib.CHILL_UNITS, None, cu.data_ptr(), None, None))
+        ms_cp = timeit(launch_cp, a.steps)
+        ms_cu = timeit(launch_cu, a.steps)
+        cols = np.unique(np.r_[np.linspace(0, C - 1, 6).astype(int), np.arange(C - 2, C)])
+        lo_s, hi_s = lo[:, cols].cpu().numpy(), hi[:, cols].cpu().numpy()
+        dl = converters.day_lengths(converters.day_angle(ta.year, ta.doy, "noleap")[:, None], lats[idx_np[cols]][None])
+        hr = CO.hourly_temperature(lo_s, hi_s, dl)
+        ocp, _, _ = CO.chill(hr, poff_j, mask, (1.0, 273.15), (1.0, 0.0))
+        _, ocu, _ = CO.chill(hr, poff, None, (1.0, 273.15), (1.0, 0.0))
+        got_cp, got_cu = cp[:, cols].cpu().numpy(), cu[:, cols].cpu().numpy()
+        sel_hours = int(mask.sum()) * 24
+        nb = 2 * T * C * 4 + Pj * C * 8
+        report(f"chill_portions (fused, 09-01..03-30, YS-JUL), {a.lat} x 1440 cells", ms_cp, nb,
+               {"selected_hours_per_cell": sel_hours, "fp64_exp_per_s": 4 * sel_hours * C / (ms_cp * 1e-3),
+                "oracle_check": {"cells": int(cols.size),
+                                 "max_rel_err": float(np.nanmax(np.abs(got_cp - ocp) / np.maximum(np.abs(ocp), 1e-300)))},
+                **card})
+        report(f"chill_units (fused, YS), {a.lat} x 1440 cells", ms_cu, 2 * T * C * 4 + P * C * 8,
+               {"oracle_check": {"cells": int(cols.size), "mismatches": int(np.sum(got_cu != ocu))}, **card})
+        del lo, hi, w, cp, cu
+        torch.cuda.empty_cache()
     if want("fwi") and a.only:      # the fire-weather kernel: opt-in (--only fwi), never part of a default run
         import time
 

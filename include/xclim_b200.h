@@ -854,6 +854,39 @@ int32_t xc_rain_season_f32(const float* x, int64_t T, int64_t C, int64_t ldx, co
                            int32_t window_dry_end, int32_t method_dry_end, int32_t* out_start, int32_t* out_end,
                            void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * c1  chill portions (Dynamic Model) and chill units (Utah Model) -- indices/_agro.py:1436-1534
+ *   `chill_portions`, :1537-1592 `chill_units`, per period of freq, on the hourly temperature of
+ *   `make_hourly_temperature` (indices/helpers.py:1059-1123).
+ *   xc_chill_daily_f32: tasmin, tasmax (T, C) daily at x[t * ldx + c], ldx >= C; the 24 hours of each day
+ *   are made in registers from weights (T, L, XC_CHILL_ROW) float64, the row of cell c being
+ *   lat_index[c] (converters.hourly_weights).  xc_chill_hourly: an explicit hourly series (H, C), float32
+ *   or float64 (x_f64), 24 steps per day from 00:00 (the last day may be partial: 24 (T - 1) < H <= 24 T).
+ *   period_offsets: (P + 1) day offsets.  day_mask: device uint8 (T), nonzero = selected, or null for
+ *   every day; unselected days are skipped (select_time(drop=True) for the portions, NaN for the units).
+ *   An hourly value v is v * k_scale + k_offset in K for the portions and v * c_scale + c_offset in degC
+ *   for the units.  what: XC_CHILL_PORTIONS | XC_CHILL_UNITS, plus XC_CHILL_POSITIVE_ONLY for the units.
+ *   out_cp, out_cu: device float64 (P, C) at out[p * C + c]; out_valid: int32 (P, C) selected non-NaN
+ *   hours, or null.  xc_hourly_temperature_f32 writes the hourly series (24 T, C) float64 at
+ *   out[h * C + c].  Semantics in xclim_b200/csrc/chill_core.cuh and DESIGN.md section 4.
+ * ------------------------------------------------------------------------------------------- */
+#define XC_CHILL_ROW 28
+#define XC_CHILL_PORTIONS 1
+#define XC_CHILL_UNITS 2
+#define XC_CHILL_POSITIVE_ONLY 4
+int32_t xc_chill_daily_f32(const float* tasmin, const float* tasmax, int64_t T, int64_t C, int64_t ldx,
+                           const double* weights, int32_t L, const int32_t* lat_index,
+                           const int32_t* period_offsets, int32_t P, const uint8_t* day_mask, double k_scale,
+                           double k_offset, double c_scale, double c_offset, int32_t what, double* out_cp,
+                           double* out_cu, int32_t* out_valid, void* stream);
+int32_t xc_chill_hourly(const void* x, int32_t x_f64, int64_t H, int64_t C, int64_t ldx,
+                        const int32_t* period_offsets, int32_t P, const uint8_t* day_mask, double k_scale,
+                        double k_offset, double c_scale, double c_offset, int32_t what, double* out_cp,
+                        double* out_cu, int32_t* out_valid, void* stream);
+int32_t xc_hourly_temperature_f32(const float* tasmin, const float* tasmax, int64_t T, int64_t C, int64_t ldx,
+                                  const double* weights, int32_t L, const int32_t* lat_index, double* out,
+                                  void* stream);
+
 #ifdef __cplusplus
 }
 #endif

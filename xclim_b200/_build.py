@@ -37,7 +37,7 @@ NVCC_FLAGS = [
 #: evapotranspiration formulas the CPU tests build for the host).
 EXTRA_FLAGS = {"fwi.cu": ["-fmad=false"], "dqm.cu": ["-fmad=false"], "stdindex.cu": ["-fmad=false"],
                "ensemble.cu": ["-fmad=false"], "evfit.cu": ["-fmad=false"], "analog.cu": ["-fmad=false"],
-               "pet.cu": ["-fmad=false"]}
+               "pet.cu": ["-fmad=false"], "chill.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:

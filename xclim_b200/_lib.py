@@ -98,6 +98,11 @@ SIGNATURES = {
     "xc_ens_moments_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "xc_ens_robustness_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64,
                                      _vp, _i32, _f64, _i32, _vp, _vp, _vp]),
+    "xc_chill_daily_f32": (_i32, [_vp, _vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _i32, _vp, _f64, _f64, _f64, _f64,
+                                  _i32, _vp, _vp, _vp, _vp]),
+    "xc_chill_hourly": (_i32, [_vp, _i32, _i64, _i64, _i64, _vp, _i32, _vp, _f64, _f64, _f64, _f64, _i32, _vp, _vp,
+                               _vp, _vp]),
+    "xc_hourly_temperature_f32": (_i32, [_vp, _vp, _i64, _i64, _i64, _vp, _i32, _vp, _vp, _vp]),
     "xc_rain_season_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _i32, _vp, C.c_float, _f64, _i32, _i32, _f64, _i32,
                                   _i32, _f64, _i32, _i32, _vp, _vp, _vp]),
 }
@@ -128,6 +133,10 @@ PET_METHODS = {"BR65": 0, "HG85": 1, "MB05": 2, "allen98": 3, "TW48": 4, "DA02":
 PET_MONTHLY = ("TW48", "DA02")
 PET_INPUTS = ("tasmin", "tasmax", "tas", "hurs", "rsds", "rsus", "rlds", "rlus", "sfcWind", "pr", "evspsblpot")
 
+
+# chill portions and units (include/xclim_b200.h c1)
+CHILL_ROW = 28
+CHILL_PORTIONS, CHILL_UNITS, CHILL_POSITIVE_ONLY = 1, 2, 4
 
 # rain season (include/xclim_b200.h r1)
 RS_METHODS = {"per_day": 0, "total": 1}

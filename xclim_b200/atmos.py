@@ -181,6 +181,9 @@ def with_missing_any(index_fn, name=None):
     return streamed(indicator)       # host-backed inputs: missing counts + index per lat slab
 
 
+from .chill import atmos_chill_portions as chill_portions, atmos_chill_units as chill_units  # noqa: E402,F401
+
+
 def _stream_fused():
     from .streaming import streamed
     g = globals()

@@ -91,11 +91,39 @@ def extraterrestrial_solar_radiation(da, lat_deg, solar_constant=1361.0):
         eccentricity_correction_factor(da)
 
 
-def day_lengths(da, lat_deg):
-    """(:450-525) in hours; NaN in polar days and nights (``infill_polar_days=False``)."""
+def day_lengths(da, lat_deg, infill_polar_days=False):
+    """(:450-525) in hours; NaN in polar days and nights, or with ``infill_polar_days`` 24 h in those north of
+    66.5 degrees (south of -66.5) with a positive (negative) declination and 0 h in the others (:510-518)."""
+    decl = solar_declination(da)
     with np.errstate(invalid="ignore"):
-        return (24 / np.pi) * np.arccos(-np.tan(np.asarray(lat_deg, dtype=np.float64) * (np.pi / 180))
-                                        * np.tan(solar_declination(da)))
+        dl = (24 / np.pi) * np.arccos(-np.tan(np.asarray(lat_deg, dtype=np.float64) * (np.pi / 180)) * np.tan(decl))
+    if infill_polar_days:
+        lat_b, decl_b = np.broadcast_arrays(np.asarray(lat_deg, dtype=np.float64), decl)
+        polar_day = ((lat_b > 66.5) & (decl_b > 0)) | ((lat_b < -66.5) & (decl_b < 0))
+        polar_night = ((lat_b > 66.5) & (decl_b < 0)) | ((lat_b < -66.5) & (decl_b > 0))
+        missing = np.isnan(dl)
+        dl = np.where(polar_day & missing, 24.0, dl)
+        dl = np.where(polar_night & missing, 0.0, dl)
+    return dl
+
+
+def hourly_weights(ta, lat_u, infill_polar_days=False):
+    """(T, L, ``_lib.CHILL_ROW``) float64 weight rows of ``make_hourly_temperature`` (indices/helpers.py
+    :1059-1123) per (day, latitude), every transcendental of the hourly profile in numpy's float64:
+    ``[0, 24)`` ``sin(pi*h / (dl + 4))`` for the day hours (``h < dl``) and ``log(clip(h + 1 - dl, 1))`` for the
+    night hours, ``[24]`` ``sin(pi*dl / (dl + 4))`` (sunset), ``[25]`` ``log(24 - (dl - 1))``, ``[26]`` ``dl``."""
+    dl = day_lengths(day_angle(ta.year, ta.doy, ta.calendar)[:, None], np.asarray(lat_u, np.float64)[None, :],
+                     infill_polar_days)[..., None]
+    h = np.arange(24, dtype=np.int64)
+    out = np.zeros(dl.shape[:2] + (_lib.CHILL_ROW,))
+    with np.errstate(invalid="ignore", divide="ignore"):
+        day = np.sin((np.pi * h) / (dl + 4))
+        night = np.log((h + 1 - dl).clip(1))
+        out[..., :24] = np.where(h < dl, day, night)
+        out[..., 24] = np.sin((np.pi * dl) / (dl + 4))[..., 0]
+        out[..., 25] = np.log(24 - (dl - 1))[..., 0]
+    out[..., 26] = dl[..., 0]
+    return out
 
 
 def _daily_table(method, ta, lat_u):

@@ -64,6 +64,14 @@ def to_time_cell(values, time_axis: int, device=None):
     return t.reshape(t.shape[0], -1), cell_shape
 
 
+def to_time_cell_f64(values, time_axis: int):
+    """:func:`to_time_cell` keeping float64: a contiguous ``(T, C)`` float64 CUDA tensor and the cell shape."""
+    _require_cuda()
+    t = values if isinstance(values, torch.Tensor) else torch.from_numpy(np.asarray(values, dtype=np.float64))
+    t = t.movedim(time_axis, 0).to("cuda" if not t.is_cuda else t.device, torch.float64).contiguous()
+    return t.reshape(t.shape[0], -1), tuple(t.shape[1:])
+
+
 _small_cache: dict = {}
 
 
@@ -767,6 +775,72 @@ def pet_monthly(inputs, moff, yoff, mdays, table, lat_index, params):
     check(load().xc_pet_monthly_f32(ptrs, T, C, ld, moff_d.data_ptr(), M, yoff_d.data_ptr(), yoff_d.numel() - 1,
                                     mdays_d.data_ptr(), table.data_ptr(), table.shape[1], lat_index.data_ptr(),
                                     ctypes.byref(params), out.data_ptr(), current_stream_ptr()))
+    return out
+
+
+# ------------------------------------------------------------------------------------ chill portions and units
+def _chill_out(P, C, what, want_valid, dev):
+    f64 = dict(dtype=torch.float64, device=dev)
+    cp = torch.empty((P, C), **f64) if what & _lib.CHILL_PORTIONS else None
+    cu = torch.empty((P, C), **f64) if what & _lib.CHILL_UNITS else None
+    valid = torch.empty((P, C), dtype=torch.int32, device=dev) if want_valid else None
+    return cp, cu, valid
+
+
+def _day_mask(day_mask, dev):
+    if day_mask is None:
+        return None
+    return torch.from_numpy(np.ascontiguousarray(day_mask, dtype=np.uint8)).to(dev)
+
+
+def chill_daily(tasmin, tasmax, weights, lat_index, poff, day_mask, to_k, to_c, what, want_valid=False):
+    """Chill portions / units per period from daily ``tasmin`` / ``tasmax`` (T, C) float32 device tensors (same
+    strides, a row stride > C works in place), the hours made in the kernel (xc_chill_daily_f32).  ``weights``
+    (T, L, CHILL_ROW) float64 device tensor, ``lat_index`` (C,) int32 device tensor, ``poff`` day offsets,
+    ``day_mask`` (T,) host bool / uint8 or None, ``to_k`` / ``to_c`` the (scale, offset) of the hourly values to K
+    and degC, ``what`` the ``_lib.CHILL_*`` bits.  Returns ``(cp, cu, valid)``: float64 (P, C) or None, and the
+    int32 (P, C) count of selected non-NaN hours (None unless ``want_valid``)."""
+    T, C = tasmin.shape
+    assert tasmax.shape == tasmin.shape and tasmax.stride() == tasmin.stride()
+    assert C == 1 or tasmin.stride(1) == 1
+    dev = tasmin.device
+    P = len(poff) - 1
+    poff_d = dev_ints(poff, np.int32, dev)
+    mask_d = _day_mask(day_mask, dev)
+    cp, cu, valid = _chill_out(P, C, what, want_valid, dev)
+    check(load().xc_chill_daily_f32(tasmin.data_ptr(), tasmax.data_ptr(), T, C, tasmin.stride(0), weights.data_ptr(),
+                                    weights.shape[1], lat_index.data_ptr(), poff_d.data_ptr(), P, _ptr(mask_d),
+                                    float(to_k[0]), float(to_k[1]), float(to_c[0]), float(to_c[1]), int(what),
+                                    _ptr(cp), _ptr(cu), _ptr(valid), current_stream_ptr()))
+    return cp, cu, valid
+
+
+def chill_hourly(x2d, poff, day_mask, to_k, to_c, what, want_valid=False):
+    """:func:`chill_daily` on an explicit hourly series ``x2d`` (H, C) float32 or float64 device tensor, 24 steps
+    per day from 00:00 (xc_chill_hourly); ``poff`` and ``day_mask`` are per day."""
+    H, C = x2d.shape
+    assert C == 1 or x2d.stride(1) == 1
+    assert x2d.dtype in (torch.float32, torch.float64)
+    dev = x2d.device
+    P = len(poff) - 1
+    poff_d = dev_ints(poff, np.int32, dev)
+    mask_d = _day_mask(day_mask, dev)
+    cp, cu, valid = _chill_out(P, C, what, want_valid, dev)
+    check(load().xc_chill_hourly(x2d.data_ptr(), int(x2d.dtype == torch.float64), H, C, x2d.stride(0),
+                                 poff_d.data_ptr(), P, _ptr(mask_d), float(to_k[0]), float(to_k[1]), float(to_c[0]),
+                                 float(to_c[1]), int(what), _ptr(cp), _ptr(cu), _ptr(valid), current_stream_ptr()))
+    return cp, cu, valid
+
+
+def hourly_temperature(tasmin, tasmax, weights, lat_index):
+    """The hourly series (24 T, C) float64 of ``make_hourly_temperature`` (xc_hourly_temperature_f32)."""
+    T, C = tasmin.shape
+    assert tasmax.shape == tasmin.shape and tasmax.stride() == tasmin.stride()
+    assert C == 1 or tasmin.stride(1) == 1
+    out = torch.empty((24 * T, C), dtype=torch.float64, device=tasmin.device)
+    check(load().xc_hourly_temperature_f32(tasmin.data_ptr(), tasmax.data_ptr(), T, C, tasmin.stride(0),
+                                           weights.data_ptr(), weights.shape[1], lat_index.data_ptr(), out.data_ptr(),
+                                           current_stream_ptr()))
     return out
 
 

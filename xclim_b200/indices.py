@@ -6,6 +6,7 @@ Same names / arguments / units as ``xclim.indices`` so that they can be bound to
 from __future__ import annotations
 
 from . import generic
+from .chill import chill_portions, chill_units, make_hourly_temperature  # noqa: F401
 from .converters import potential_evapotranspiration, water_budget  # noqa: F401
 from .units import threshold_in_units_of
 
