@@ -687,6 +687,45 @@ def main():
                {"oracle_check": {"cells": int(cols.size), "mismatches": int(np.sum(got_cu != ocu))}, **card})
         del lo, hi, w, cp, cu
         torch.cuda.empty_cache()
+    if want("bootspell") and a.only:   # bootstrapped WSDI: opt-in (--only bootspell), on the --lat band
+        import subprocess
+
+        from torch.profiler import ProfilerActivity, profile
+        sys.path.insert(0, os.path.join(ROOT, "tests"))
+        import fake_bootstrap   # the oracle-backed restatement of xc_bootstrap_doy_index_f32 (CPU)
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True)
+        card = {"gpu": torch.cuda.get_device_name(), "power_limit": q.stdout.strip() or "unknown"}
+        # warm_spell_duration_index(window=6, bootstrap=True) at per 90 over a 15-year base starting the series:
+        # the bootstrapped periods of the base years, next to tx90p(bootstrap=True)'s count on the same input
+        NB = 15
+        sp = np.repeat(np.arange(NB), YEAR).astype(np.int32)
+        P = T // YEAR
+        gt = _lib.OPS[">"]
+
+        def spell():
+            return device.bootstrap_doy_index(tas, 0, NB, YEAR, sp, P, 5, 90.0, 1 / 3, 1 / 3, gt, "spell", 6)[0]
+
+        def count():
+            return device.bootstrap_doy_count(tas, 0, NB, YEAR, sp, P, 5, 90.0, 1 / 3, 1 / 3, gt)
+        ms_spell = timeit(spell, a.steps)
+        ms_count = timeit(count, a.steps)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            got = spell()
+            torch.cuda.synchronize()
+        kern = {}
+        for e in prof.key_averages():
+            for k in ("bootstrap5_kernel", "bootstrap_kernel", "bootstrap_reduce_kernel"):
+                if k in e.key:
+                    kern[k] = kern.get(k, 0.0) + e.device_time_total / 1000.0
+        cols = np.unique(np.r_[np.linspace(0, C - 1, 2).astype(int), C - 1])
+        xs = torch.from_numpy(tas[:NB * YEAR, cols].cpu().numpy())
+        exp, _ = fake_bootstrap.bootstrap_doy_index(xs, 0, NB, YEAR, sp, P, 5, 90.0, 1 / 3, 1 / 3, gt, "spell", 6)
+        ok = bool(np.array_equal(got[:NB, cols].cpu().numpy(), exp[:NB].numpy()))
+        report(f"warm_spell_duration_index(window=6, bootstrap=True), 15-year base, {a.lat} x 1440 cells", ms_spell,
+               NB * YEAR * C * 4 + NB * C * 8,
+               {"ms_bootstrap_doy_count_same_input": ms_count, "ratio_to_count": ms_spell / ms_count,
+                "kernel_ms": kern, "oracle_check": {"cells": int(cols.size), "bit_exact": ok}, **card})
     if want("fwi") and a.only:      # the fire-weather kernel: opt-in (--only fwi), never part of a default run
         import time
 

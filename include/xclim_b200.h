@@ -75,6 +75,11 @@ extern "C" {
 #define XC_TF_EXCESS 1  /* (x - thr).clip(0) for >,>= ; (thr - x).clip(0) for <,<= : generic.py:1514-1552 */
 #define XC_TF_WHERE 2   /* x where (x op thr) else NaN: generic.py:1278-1320 (`thresholded_statistics`) */
 
+/* per-replacement indices of xc_bootstrap_doy_index_f32 */
+#define XC_BOOT_COUNT 0  /* days_over_precip_thresh: indices/_multivariate.py:1174-1233 */
+#define XC_BOOT_SPELL 1  /* warm / cold spell duration index: indices/_multivariate.py:69-153, 1719-1795 */
+#define XC_BOOT_SUM 2    /* fraction_over_precip_thresh: indices/_multivariate.py:1238-1297 */
+
 int32_t xc_version(void);
 const char* xc_last_error(void);
 
@@ -375,6 +380,35 @@ int32_t xc_bootstrap_doy_count_f32(const float* x, int64_t T, int64_t C, int64_t
                                    const int32_t* step_period, int32_t P,
                                    int32_t window, double percentile, double alpha, double beta,
                                    int32_t op, int32_t* count_scratch, double* out, void* stream);
+
+/* The same bootstrap for the indices whose value depends on the ORDER of the exceedance days or on the values
+ * over the threshold -- `percentile_bootstrap` on warm_spell_duration_index, cold_spell_duration_index,
+ * days_over_precip_thresh and fraction_over_precip_thresh (indices/_multivariate.py:69-153, 1174-1297, 1719-1795;
+ * core/bootstrapping.py:81-211, 235-282).  For every in-base year y and base year s != y the bootstrap kernel
+ * writes year y's exceedance mask against max(P^(y<-s), floor) (a NaN percentile takes the floor:
+ * `pr_per.where(pr_per > thresh, thresh)`, :1222, 1288; floor = -inf: no floor, a NaN percentile is never
+ * exceeded), then one lane per (cell, y) computes the index on year y's own slice for each s and averages:
+ *   XC_BOOT_COUNT: out float64 (P, C), mean over s of the days over the threshold;
+ *   XC_BOOT_SPELL: out float64 (P, C), mean over s of rl.windowed_run_count(mask, run_window) per period
+ *                  (resample_before_rl as in xc_doy_runstat_f32; runs end at the edges of year y);
+ *   XC_BOOT_SUM:   out float32 (P, C), mean over s of float32(float64 time-order sum of x over the mask days)
+ *                  / wet_total[p, c] (float32 (P, C), row stride C): the float64 sum of the non-NaN float32
+ *                  fractions in s order over their number, rounded once to float32; NaN when all are NaN.
+ * Only periods holding base steps are written.  floor is only accepted with > / >=.
+ * step_period must keep every period inside one base year (the periods nest in the years: one lane per (cell,
+ * year) writes a period's result); a period spanning two years is not detected and gives undefined results.
+ * scratch: device memory of scratch_bytes bytes, 16-byte aligned.  The cells are processed in tiles of as many
+ * cells as it holds masks for (xc_bootstrap_doy_index_scratch_bytes(N, L, C) bytes: all of them); a tile smaller
+ * than the C and than 128 cells is XC_ERR_INVALID.  On return the scratch holds the last tile's masks,
+ * uint32 [(pair * ceil(L / 32) + d / 32) * n + c], pair = y (N - 1) + (s < y ? s : s - 1), n its cells. */
+int64_t xc_bootstrap_doy_index_scratch_bytes(int32_t n_base_years, int32_t year_len, int64_t C);
+int32_t xc_bootstrap_doy_index_f32(const float* x, int64_t T, int64_t C, int64_t ldx,
+                                   int64_t base_start, int32_t n_base_years, int32_t year_len,
+                                   const int32_t* step_period, int32_t P,
+                                   int32_t window, double percentile, double alpha, double beta, int32_t op,
+                                   int32_t reducer, int32_t run_window, int32_t resample_before_rl, double floor,
+                                   const float* wet_total, void* scratch, int64_t scratch_bytes, void* out,
+                                   void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * a20  empirical quantile mapping -- xsdba.EmpiricalQuantileMapping (third-party, re-exported

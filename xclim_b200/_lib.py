@@ -60,6 +60,9 @@ SIGNATURES = {
     "xc_period_range_stat_f32": (_i32, [_vp, _vp, _i64, _i64, _i64, _vp, _i32, _i32, _i32, _vp, _vp]),
     "xc_bootstrap_doy_count_f32": (_i32, [_vp, _i64, _i64, _i64, _i64, _i32, _i32, _vp, _i32, _i32, _f64, _f64,
                                           _f64, _i32, _vp, _vp, _vp]),
+    "xc_bootstrap_doy_index_scratch_bytes": (_i64, [_i32, _i32, _i64]),
+    "xc_bootstrap_doy_index_f32": (_i32, [_vp, _i64, _i64, _i64, _i64, _i32, _i32, _vp, _i32, _i32, _f64, _f64, _f64,
+                                          _i32, _i32, _i32, _i32, _f64, _vp, _vp, _i64, _vp, _vp]),
     "xc_eqm_train_workspace_bytes": (_i64, [_i64, _i64, _i32]),
     "xc_eqm_train_f32": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _i64, _vp]),
     "xc_eqm_adjust_f32": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),

@@ -16,11 +16,17 @@
 // insertions into a short list and one lerp remain.  Counts are accumulated per output period with
 // integer atomics and divided by N-1 at the end (mean over the N-1 altered series,
 // core/bootstrapping.py:203; numpy's int64 mean is exactly sum/(N-1) in float64).
+//
+// The same kernels in MASK mode keep the (y, s) identity instead: they set bit d of year y's mask word for pair
+// (y, s) when day d beats P^(y<-s)(d), and bootstrap_reduce_kernel turns the masks into the spell and sum indices
+// (bootstrap_reduce_core.cuh).  Their day chunks start on multiples of 32 days, so that each mask word has one
+// writing thread and a plain read-modify-write after the memset needs no atomics.
 #include <stdlib.h>
 
 #include <type_traits>
 #include <vector>
 
+#include "bootstrap_reduce_core.cuh"
 #include "common.cuh"
 #include "quantile.cuh"
 #include "sortnet.cuh"
@@ -29,6 +35,33 @@ namespace xc {
 namespace {
 
 constexpr int kThreads = 128;
+
+// output of the exceedance kernels: per-period counts (tx90p & family) or per-(y, s) day masks
+constexpr int kCount = 0, kMask = 1;
+
+// MASK mode: mask [N (N - 1)][Wd][C] words, floor the threshold floor (-inf: none)
+struct MaskOut {
+  uint32_t* mask;
+  int32_t Wd;
+  double floor;
+};
+__device__ __forceinline__ bool has_floor(double floor) { return floor > (double)XC_NEG_INF; }
+// max(P, floor), a NaN percentile taking the floor (`pr_per.where(pr_per > thresh, thresh)`); no floor: P
+__device__ __forceinline__ double floored(double p, double floor) {
+  return (has_floor(floor) && !(p > floor)) ? floor : p;
+}
+__device__ __forceinline__ void set_pair_bit(const MaskOut& mo, int64_t C, int64_t c, int N, int y, int s, int d) {
+  const int64_t pair = (int64_t)y * (N - 1) + (s < y ? s : s - 1);
+  uint32_t* w = mo.mask + (pair * mo.Wd + (d >> 5)) * C + c;
+  *w |= 1u << (d & 31);
+}
+// x beats P^(y<-s) for every s: the mask bit is x op floor (x op max(P, f) == x op P && x op f for > / >=)
+template <int OP>
+__device__ __forceinline__ void set_year_bits(const MaskOut& mo, int64_t C, int64_t c, int N, int y, int d, double x) {
+  if (has_floor(mo.floor) && !cmpd<OP>(x, mo.floor)) return;
+  for (int s = 0; s < N; ++s)
+    if (s != y) set_pair_bit(mo, C, c, N, y, s, d);
+}
 
 // remove ONE instance of value r from the sorted list (no-op when absent; NaN never matches)
 template <int K>
@@ -91,11 +124,11 @@ __device__ __noinline__ float altered_max(const float* raw, int stride, int raw_
 //   sring [W-1][KA]  sorted (selection-side, masked) extremes of the W-1 previous day lists
 //   scnt  [W-1]      their valid counts
 //   raw   [W][N]     raw block values x[base + b*L + dd] of the W days of the current window
-template <int KA, int KB, int OP>
+template <int KA, int KB, int OP, int MODE>
 __global__ void __launch_bounds__(kThreads)
 bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t base_start, int32_t N, int32_t L,
                  int32_t W, QuantSpec spec, const int32_t* __restrict__ step_period, int32_t doys_per_chunk,
-                 int32_t* __restrict__ counts) {
+                 int32_t* __restrict__ counts, MaskOut mo) {
   extern __shared__ float smem[];
   const int H = W / 2, R = W - 1;
   const int lane = threadIdx.x;
@@ -223,7 +256,8 @@ bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t ba
           decided = true;                       // never beats the threshold
         } else if (geT < KA && geA + W <= k1min) {
           decided = true;                       // beats it for every other year s
-          atomicAdd(counts + (int64_t)step_period[y * L + d] * C + c, N - 1);
+          if constexpr (MODE == kCount) atomicAdd(counts + (int64_t)step_period[y * L + d] * C + c, N - 1);
+          else set_year_bits<OP>(mo, C, c, N, y, d, (double)xq);
         }
       }
       if (!decided) band |= (N <= 32) ? (1u << y) : 0u;
@@ -277,7 +311,8 @@ bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t ba
         }
         double p = finalize_quantile<KB>(bl, nm, spec);
         if (lerp_is_nan(p, nm)) p = altered_max(raw + lane, kThreads, raw_first, W, N, L, d, y, s, vmask, 1.f);
-        cnt += cmpd<OP>((double)xq, p) ? 1 : 0;
+        if constexpr (MODE == kCount) cnt += cmpd<OP>((double)xq, p) ? 1 : 0;
+        else if (cmpd<OP>((double)xq, floored(p, mo.floor))) set_pair_bit(mo, C, c, N, y, s, d);
       }
       if (cnt) atomicAdd(counts + (int64_t)step_period[y * L + d] * C + c, cnt);
     }
@@ -349,11 +384,11 @@ __device__ __forceinline__ float pick16(const float (&l)[16], int idx) {
   return (idx & 8) ? u1 : u0;
 }
 
-template <int OP>
+template <int OP, int MODE>
 __global__ void __launch_bounds__(kBT)
 bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t base_start, int32_t N, int32_t L,
                   QuantSpec spec, const int32_t* __restrict__ step_period, int32_t doys_per_chunk,
-                  int32_t* __restrict__ counts) {
+                  int32_t* __restrict__ counts, MaskOut mo) {
   constexpr int KA = 16, KB = 8, W = 5, H = 2;
   extern __shared__ float smem[];
   const int lane = threadIdx.x;
@@ -480,7 +515,8 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
       const float xs = raw[((size_t)raw_mid * N + y) * kBT + lane];
       if (xs == xs) {
         if (xs > thr_always) {
-          atomicAdd(counts + (int64_t)step_period[y * L + d] * C + c, N - 1);
+          if constexpr (MODE == kCount) atomicAdd(counts + (int64_t)step_period[y * L + d] * C + c, N - 1);
+          else set_year_bits<OP>(mo, C, c, N, y, d, (double)(sgn * xs));
         } else if (!(xs < thr_never)) {
           maybe |= 1u << y;
         }
@@ -530,7 +566,8 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
           decided = true;
         } else if (gmax >= 0 && xs > ta) {
           decided = true;
-          atomicAdd(counts + (int64_t)step_period[y * L + d] * C + c, N - 1);
+          if constexpr (MODE == kCount) atomicAdd(counts + (int64_t)step_period[y * L + d] * C + c, N - 1);
+          else set_year_bits<OP>(mo, C, c, N, y, d, (double)(sgn * xs));
         }
       }
       if (!decided) band |= (1u << y);
@@ -588,7 +625,11 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
           deep |= (stop[((size_t)2 * N + s) * kBT + lane] > b0) ? (1u << s) : 0u;   // three or more values above a[k1+1]
         }
         const unsigned others = all & ~(1u << y) & ~nanmask;
-        cnt = t0 * __popc(others & ~owners);
+        if constexpr (MODE == kCount) {
+          cnt = t0 * __popc(others & ~owners);
+        } else if (cmpd<OP>((double)xq, floored(p0, mo.floor))) {
+          for (unsigned m = others & ~owners; m; m &= m - 1u) set_pair_bit(mo, C, c, N, y, __ffs(m) - 1, d);
+        }
         unsigned todo = others & owners & ~deep;
         unsigned full = others & deep;
         slow = all & ~(1u << y) & nanmask;
@@ -599,7 +640,8 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
           const float uhi = fmaxf(b1, fmaxf(fminf(b2, i1), fminf(b3, i2)));
           const float ulo = fmaxf(b0, fmaxf(fminf(b1, i1), fminf(b2, i2)));
           const double p = top ? quant_lerp(ulo, uhi, qm) : quant_lerp(-uhi, -ulo, qm);
-          cnt += cmpd<OP>((double)xq, p) ? 1 : 0;
+          if constexpr (MODE == kCount) cnt += cmpd<OP>((double)xq, p) ? 1 : 0;
+          else if (cmpd<OP>((double)xq, floored(p, mo.floor))) set_pair_bit(mo, C, c, N, y, s, d);
         }
         while (full) {     // rare: the whole sorted window
           const int s = __ffs(full) - 1;
@@ -613,7 +655,8 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
           const float ulo = fmaxf(fmaxf(fmaxf(b0, fminf(b1, j1)), fmaxf(fminf(b2, j2), fminf(b3, j3))),
                                   fmaxf(fminf(b4, j4), fminf(b5, j5)));
           const double p = top ? quant_lerp(ulo, uhi, qm) : quant_lerp(-uhi, -ulo, qm);
-          cnt += cmpd<OP>((double)xq, p) ? 1 : 0;
+          if constexpr (MODE == kCount) cnt += cmpd<OP>((double)xq, p) ? 1 : 0;
+          else if (cmpd<OP>((double)xq, floored(p, mo.floor))) set_pair_bit(mo, C, c, N, y, s, d);
         }
       }
       while (slow) {   // insert-and-finalize (bootstrap_kernel's exact step)
@@ -633,7 +676,8 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
         }
         double p = finalize_quantile<KB>(bl, nm, spec);
         if (lerp_is_nan(p, nm)) p = altered_max(raw + lane, kBT, raw_first, W, N, L, d, y, s, vmask, sgn);
-        cnt += cmpd<OP>((double)xq, p) ? 1 : 0;
+        if constexpr (MODE == kCount) cnt += cmpd<OP>((double)xq, p) ? 1 : 0;
+        else if (cmpd<OP>((double)xq, floored(p, mo.floor))) set_pair_bit(mo, C, c, N, y, s, d);
       }
       if (cnt) atomicAdd(counts + (int64_t)step_period[y * L + d] * C + c, cnt);
     }
@@ -641,20 +685,24 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
   }
 }
 
+template <int MODE>
 int32_t launch_bootstrap5(int32_t op, const float* x, int64_t C, int64_t ldx, int64_t base_start, int32_t N, int32_t L,
-                          const QuantSpec& spec, const int32_t* step_period, int32_t* counts, cudaStream_t st) {
+                          const QuantSpec& spec, const int32_t* step_period, int32_t* counts, const MaskOut& mo,
+                          cudaStream_t st) {
   const int64_t cblocks = (C + kBT - 1) / kBT;
-  const DaySplit sp = split_days(L, cblocks, 12, 20, false);
+  const DaySplit sp = split_days(L, cblocks, 12, 20, false, MODE == kMask ? 32 : 1);
   const size_t smem = ((size_t)8 * N + 16) * kBT * 4;
   if (smem > 227 * 1024) return 1;
   dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
   return dispatch_op(op, [&](auto OPC) -> int32_t {
     constexpr int OP = decltype(OPC)::value;
     if (smem > 48 * 1024) {
-      cudaError_t e = cudaFuncSetAttribute(bootstrap5_kernel<OP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      cudaError_t e = cudaFuncSetAttribute(bootstrap5_kernel<OP, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)smem);
       if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(bootstrap5_kernel)");
     }
-    bootstrap5_kernel<OP><<<grid, kBT, smem, st>>>(x, C, ldx, base_start, N, L, spec, step_period, sp.per, counts);
+    bootstrap5_kernel<OP, MODE><<<grid, kBT, smem, st>>>(x, C, ldx, base_start, N, L, spec, step_period, sp.per,
+                                                         counts, mo);
     return launch_status("bootstrap5_kernel");
   });
 }
@@ -665,12 +713,12 @@ bootstrap_finish_kernel(const int32_t* __restrict__ counts, int64_t n, double de
   if (i < n) out[i] = (double)counts[i] / denom;
 }
 
-template <int KA, int KB>
+template <int KA, int KB, int MODE>
 int32_t launch_bootstrap(int32_t op, const float* x, int64_t C, int64_t ldx, int64_t base_start, int32_t N,
                          int32_t L, int32_t W, const QuantSpec& spec, const int32_t* step_period, int32_t* counts,
-                         cudaStream_t st) {
+                         const MaskOut& mo, cudaStream_t st) {
   const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  const DaySplit sp = split_days(L, cblocks, 6, 4 * W, false);
+  const DaySplit sp = split_days(L, cblocks, 6, 4 * W, false, MODE == kMask ? 32 : 1);
   const size_t smem = ((size_t)(W - 1) * (KA + 1) + (size_t)W * N) * kThreads * 4;
   if (smem > 227 * 1024) {
     set_error("bootstrap: %d base years x window %d need %zu bytes of shared memory per block", N, W, smem);
@@ -680,14 +728,64 @@ int32_t launch_bootstrap(int32_t op, const float* x, int64_t C, int64_t ldx, int
   return dispatch_op(op, [&](auto OPC) -> int32_t {
     constexpr int OP = decltype(OPC)::value;
     if (smem > 48 * 1024) {
-      cudaError_t e = cudaFuncSetAttribute(bootstrap_kernel<KA, KB, OP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)smem);
+      cudaError_t e = cudaFuncSetAttribute(bootstrap_kernel<KA, KB, OP, MODE>,
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(bootstrap_kernel)");
     }
-    bootstrap_kernel<KA, KB, OP><<<grid, kThreads, smem, st>>>(x, C, ldx, base_start, N, L, W, spec, step_period,
-                                                               sp.per, counts);
+    bootstrap_kernel<KA, KB, OP, MODE><<<grid, kThreads, smem, st>>>(x, C, ldx, base_start, N, L, W, spec,
+                                                                     step_period, sp.per, counts, mo);
     return launch_status("bootstrap_kernel");
   });
+}
+
+// The exceedance kernel for `need` order statistics of the window-W sample: the same choice in both modes
+template <int MODE>
+int32_t launch_exceedance(const float* x, int64_t C, int64_t ldx, int64_t base_start, int32_t N, int32_t L,
+                          int32_t window, double percentile, double alpha, double beta, int32_t op,
+                          const int32_t* step_period, int32_t* counts, const MaskOut& mo, cudaStream_t st) {
+  QuantSpec spec;
+  const int need = plan_quantile(percentile, alpha, beta, N * window, &spec);
+  int32_t e = 1;
+  if (need > 0 && need <= 8 && window == 5 && N <= 16 && L > 8 && !getenv("XCLIM_B200_BOOT_V1"))
+    e = launch_bootstrap5<MODE>(op, x, C, ldx, base_start, N, L, spec, step_period, counts, mo, st);
+  if (e != 1) {
+  } else if (need > 0 && need <= 8 && need + window <= 16)
+    e = launch_bootstrap<16, 8, MODE>(op, x, C, ldx, base_start, N, L, window, spec, step_period, counts, mo, st);
+  else if (need > 0 && need <= 16 && need + window <= 32)
+    e = launch_bootstrap<32, 16, MODE>(op, x, C, ldx, base_start, N, L, window, spec, step_period, counts, mo, st);
+  else if (need > 0 && need + window <= 32)
+    e = launch_bootstrap<32, 32, MODE>(op, x, C, ldx, base_start, N, L, window, spec, step_period, counts, mo, st);
+  else {
+    set_error("bootstrap: percentile %g of %d samples needs %d order statistics (+%d removals); at most 32 are kept",
+              percentile, N * window, need, window);
+    return XC_ERR_UNSUPPORTED;
+  }
+  return e;
+}
+
+// One lane per (cell, in-base year y = blockIdx.y): year y's index against each altered table, averaged
+// (bootstrap_reduce_core.cuh).  mask: [N (N - 1)][Wd][C]; x, wet, out: the tile's first cell, rows ldx / ldo apart.
+template <int RED>
+__global__ void __launch_bounds__(kThreads)
+bootstrap_reduce_kernel(const uint32_t* __restrict__ mask, int64_t C, int32_t Wd, int32_t N, int32_t L,
+                        const int32_t* __restrict__ step_period, int32_t window, int32_t after,
+                        const float* __restrict__ x, int64_t ldx, int64_t base_start,
+                        const float* __restrict__ wet, int64_t ldo, void* __restrict__ out) {
+  const int64_t c = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+  if (c >= C) return;
+  const int y = blockIdx.y;
+  const float* xy = x + (base_start + (int64_t)y * L) * ldx + c;
+  auto word = [&](int pair, int w) { return __ldg(mask + ((int64_t)pair * Wd + w) * C + c); };
+  auto xval = [&](int d) { return __ldg(xy + (int64_t)d * ldx); };
+  auto wetp = [&](int p) { return __ldg(wet + (int64_t)p * ldo + c); };
+  auto store_int = [&](int p, long long isum) {
+    static_cast<double*>(out)[(int64_t)p * ldo + c] = boot_int_mean(isum, N);
+  };
+  auto store_frac = [&](int p, double fsum, int nf) {
+    static_cast<float*>(out)[(int64_t)p * ldo + c] = boot_frac_mean(fsum, nf);
+  };
+  boot_reduce_year<RED>(N, L, y, step_period + (int64_t)y * L, window, after != 0, word, xval, wetp, store_int,
+                        store_frac);
 }
 
 }  // namespace
@@ -708,30 +806,77 @@ extern "C" int32_t xc_bootstrap_doy_count_f32(const float* x, int64_t T, int64_t
   XC_REQUIRE(op == XC_OP_GT || op == XC_OP_GE || op == XC_OP_LT || op == XC_OP_LE,
              "Operation `%d` not permitted for indice.", op);
   cudaStream_t st = (cudaStream_t)stream;
-  QuantSpec spec;
-  const int need = plan_quantile(percentile, alpha, beta, n_base_years * window, &spec);
   XC_CHECK_CUDA(cudaMemsetAsync(count_scratch, 0, (size_t)P * C * 4, st));
-  int32_t e = 1;
-  if (need > 0 && need <= 8 && window == 5 && n_base_years <= 16 && year_len > 8 && !getenv("XCLIM_B200_BOOT_V1"))
-    e = launch_bootstrap5(op, x, C, ldx, base_start, n_base_years, year_len, spec, step_period, count_scratch, st);
-  if (e != 1) {
-  } else if (need > 0 && need <= 8 && need + window <= 16)
-    e = launch_bootstrap<16, 8>(op, x, C, ldx, base_start, n_base_years, year_len, window, spec, step_period,
-                                count_scratch, st);
-  else if (need > 0 && need <= 16 && need + window <= 32)
-    e = launch_bootstrap<32, 16>(op, x, C, ldx, base_start, n_base_years, year_len, window, spec, step_period,
-                                 count_scratch, st);
-  else if (need > 0 && need + window <= 32)
-    e = launch_bootstrap<32, 32>(op, x, C, ldx, base_start, n_base_years, year_len, window, spec, step_period,
-                                 count_scratch, st);
-  else {
-    set_error("bootstrap: percentile %g of %d samples needs %d order statistics (+%d removals); at most 32 are kept",
-              percentile, n_base_years * window, need, window);
-    return XC_ERR_UNSUPPORTED;
-  }
+  const int32_t e = launch_exceedance<kCount>(x, C, ldx, base_start, n_base_years, year_len, window, percentile, alpha,
+                                              beta, op, step_period, count_scratch, MaskOut{nullptr, 0, 0.0}, st);
   if (e) return e;
   const int64_t n = (int64_t)P * C;
   bootstrap_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(count_scratch, n, (double)(n_base_years - 1),
                                                                       out);
   return launch_status("bootstrap_finish_kernel");
+}
+
+static int64_t mask_bytes_per_cell(int32_t N, int32_t L) { return (int64_t)N * (N - 1) * ((L + 31) / 32) * 4; }
+
+extern "C" int64_t xc_bootstrap_doy_index_scratch_bytes(int32_t n_base_years, int32_t year_len, int64_t C) {
+  if (n_base_years < 2 || year_len < 1 || C < 1) return 0;
+  return mask_bytes_per_cell(n_base_years, year_len) * C;
+}
+
+extern "C" int32_t xc_bootstrap_doy_index_f32(const float* x, int64_t T, int64_t C, int64_t ldx, int64_t base_start,
+                                              int32_t n_base_years, int32_t year_len, const int32_t* step_period,
+                                              int32_t P, int32_t window, double percentile, double alpha,
+                                              double beta, int32_t op, int32_t reducer, int32_t run_window,
+                                              int32_t resample_before_rl, double floor, const float* wet_total,
+                                              void* scratch, int64_t scratch_bytes, void* out, void* stream) {
+  XC_REQUIRE(x && step_period && scratch && out, "null pointer argument");
+  XC_REQUIRE(T > 0 && C > 0 && ldx >= C && P > 0, "bad shape");
+  XC_REQUIRE(n_base_years >= 2 && year_len >= 1, "bootstrap needs at least two base years");
+  XC_REQUIRE(base_start >= 0 && base_start + (int64_t)n_base_years * year_len <= T, "base period outside the series");
+  XC_REQUIRE(window >= 1 && window % 2 == 1 && window <= 31 && window <= year_len, "window must be odd and <= 31");
+  XC_REQUIRE(op == XC_OP_GT || op == XC_OP_GE || op == XC_OP_LT || op == XC_OP_LE,
+             "Operation `%d` not permitted for indice.", op);
+  XC_REQUIRE(reducer == XC_BOOT_COUNT || reducer == XC_BOOT_SPELL || reducer == XC_BOOT_SUM,
+             "unknown bootstrap index %d", reducer);
+  XC_REQUIRE(reducer != XC_BOOT_SPELL || run_window >= 1, "run window must be >= 1");
+  XC_REQUIRE(!(floor != floor), "floor must not be NaN");
+  XC_REQUIRE(floor == (double)-INFINITY || op == XC_OP_GT || op == XC_OP_GE, "a threshold floor needs op > or >=");
+  XC_REQUIRE((wet_total != nullptr) == (reducer == XC_BOOT_SUM), "wet_total is given exactly for XC_BOOT_SUM");
+  XC_REQUIRE(((uintptr_t)scratch & 15) == 0, "scratch must be 16-byte aligned");
+  const int32_t N = n_base_years, L = year_len, Wd = (L + 31) / 32;
+  const int64_t per_cell = mask_bytes_per_cell(N, L);
+  const int64_t fit = scratch_bytes > 0 ? scratch_bytes / per_cell : 0;
+  const int64_t tile = fit >= C ? C : fit / kThreads * kThreads;
+  XC_REQUIRE(tile > 0, "scratch of %lld bytes holds the masks of %lld cells; a tile needs %lld (%lld bytes per cell)",
+             (long long)scratch_bytes, (long long)fit, (long long)(C < kThreads ? C : kThreads), (long long)per_cell);
+  cudaStream_t st = (cudaStream_t)stream;
+  uint32_t* mask = static_cast<uint32_t*>(scratch);
+  const size_t osz = reducer == XC_BOOT_SUM ? 4 : 8;
+  for (int64_t c0 = 0; c0 < C; c0 += tile) {
+    const int64_t n = C - c0 < tile ? C - c0 : tile;
+    XC_CHECK_CUDA(cudaMemsetAsync(mask, 0, (size_t)(per_cell * n), st));
+    int32_t e = launch_exceedance<kMask>(x + c0, n, ldx, base_start, N, L, window, percentile, alpha, beta, op,
+                                         step_period, nullptr, MaskOut{mask, Wd, floor}, st);
+    if (e) return e;
+    dim3 grid((unsigned)((n + kThreads - 1) / kThreads), (unsigned)N, 1);
+    const float* wet = wet_total ? wet_total + c0 : nullptr;
+    void* o = static_cast<char*>(out) + (size_t)c0 * osz;
+    const int after = resample_before_rl ? 0 : 1;
+    switch (reducer) {
+      case XC_BOOT_COUNT:
+        bootstrap_reduce_kernel<XC_BOOT_COUNT><<<grid, kThreads, 0, st>>>(mask, n, Wd, N, L, step_period, run_window,
+                                                                          after, x + c0, ldx, base_start, wet, C, o);
+        break;
+      case XC_BOOT_SPELL:
+        bootstrap_reduce_kernel<XC_BOOT_SPELL><<<grid, kThreads, 0, st>>>(mask, n, Wd, N, L, step_period, run_window,
+                                                                          after, x + c0, ldx, base_start, wet, C, o);
+        break;
+      default:
+        bootstrap_reduce_kernel<XC_BOOT_SUM><<<grid, kThreads, 0, st>>>(mask, n, Wd, N, L, step_period, run_window,
+                                                                        after, x + c0, ldx, base_start, wet, C, o);
+    }
+    e = launch_status("bootstrap_reduce_kernel");
+    if (e) return e;
+  }
+  return XC_OK;
 }

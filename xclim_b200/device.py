@@ -354,6 +354,42 @@ def bootstrap_doy_count(x2d, base_start, n_base_years, year_len, step_period, P,
     return out
 
 
+BOOT_INDEX = {"count": 0, "spell": 1, "sum": 2}     # XC_BOOT_COUNT / SPELL / SUM
+
+
+def bootstrap_doy_index(x2d, base_start, n_base_years, year_len, step_period, P, window, percentile, alpha, beta,
+                        op_code, kind, run_window=1, resample_before_rl=True, floor=None, wet_total=None,
+                        scratch_bytes=None):
+    """(P, C) bootstrapped index of the in-base periods (xc_bootstrap_doy_index_f32): ``kind`` "count" / "spell"
+    (float64) or "sum" (float32, with the float32 (P, C) ``wet_total``); other periods are NaN.  ``floor``: the
+    threshold floor of the precipitation indices.  ``scratch_bytes`` caps the mask buffer (default: every cell's
+    masks, or a quarter of the free device memory when that is less)."""
+    T, C = x2d.shape
+    sp = dev_ints(step_period, np.int32, x2d.device)
+    assert sp.numel() == n_base_years * year_len
+    lib = load()
+    need = int(lib.xc_bootstrap_doy_index_scratch_bytes(int(n_base_years), int(year_len), C))
+    if scratch_bytes is None:
+        scratch_bytes = need
+        if x2d.is_cuda:
+            scratch_bytes = min(need, torch.cuda.mem_get_info(x2d.device)[0] // 4)
+    scratch = torch.empty(max(int(scratch_bytes), 16), dtype=torch.uint8, device=x2d.device)
+    dt = torch.float32 if kind == "sum" else torch.float64
+    out = torch.full((P, C), float("nan"), dtype=dt, device=x2d.device)
+    wet = None
+    if kind == "sum":
+        assert wet_total.dtype == torch.float32 and wet_total.shape == (P, C) and wet_total.is_contiguous()
+        wet = wet_total
+    check(lib.xc_bootstrap_doy_index_f32(x2d.data_ptr(), T, C, x2d.stride(0), int(base_start), int(n_base_years),
+                                         int(year_len), sp.data_ptr(), P, int(window), float(percentile),
+                                         float(alpha), float(beta), op_code, BOOT_INDEX[kind], int(run_window),
+                                         int(bool(resample_before_rl)),
+                                         float("-inf") if floor is None else float(floor), _ptr(wet),
+                                         scratch.data_ptr(), int(scratch_bytes), out.data_ptr(),
+                                         current_stream_ptr()))
+    return out, scratch
+
+
 # ------------------------------------------------------------------------------------ rolling / spells
 def rolling_period_reduce(x2d, poff, window, window_stat_code, center, stat_code):
     T, C = x2d.shape

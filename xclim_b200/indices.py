@@ -111,7 +111,10 @@ def days_over_precip_thresh(pr, pr_per, thresh="1 mm/day", freq="YS", bootstrap=
     indices/_multivariate.py:1176-1233: ``tp = pr_per.where(pr_per > thresh, thresh)`` then the tx90p
     count; the clamp is applied to the per-doy table on the device."""
     if bootstrap:
-        raise NotImplementedError("days_over_precip_thresh(bootstrap=True) is not supported by the xclim_b200 hot path")
+        from .bootstrapping import _check_provenance, bootstrap_doy_index
+        _check_provenance(pr_per)
+        thr = threshold_in_units_of(thresh, pr) if isinstance(thresh, str) else float(thresh)
+        return bootstrap_doy_index(pr, pr_per, freq, op, (">", ">="), "count", floor=thr)
     thr = threshold_in_units_of(thresh, pr) if isinstance(thresh, str) else float(thresh)
     return _percentile_day_count(pr, pr_per, freq, False, op, (">", ">="), floor=thr)
 
@@ -156,7 +159,8 @@ def _spell_duration_index(da, per, window, freq, resample_before_rl, bootstrap, 
     from .field import attrs_of
     from .generic import _unwrap, _wrap_periods
     if bootstrap:
-        raise NotImplementedError(f"{name}(bootstrap=True) is not supported by the xclim_b200 hot path")
+        from .bootstrapping import bootstrap_doy_index
+        return bootstrap_doy_index(da, per, freq, op, constrain, "spell", int(window), resample_before_rl)
     code = _lib.op_code(op, constrain)
     x2d, cell_shape, other, ta = _unwrap(da)
     table, doy_idx = _doy_table(per, da, x2d, cell_shape, other, ta)
@@ -194,8 +198,10 @@ def fraction_over_precip_thresh(pr, pr_per, thresh="1 mm/day", freq="YS", bootst
     from .field import attrs_of, dims_of
     from .generic import _array_threshold, _unwrap, _wrap_periods
     if bootstrap:
-        raise NotImplementedError("fraction_over_precip_thresh(bootstrap=True) is not supported by the xclim_b200 "
-                                  "hot path")
+        from .bootstrapping import _check_provenance, bootstrap_doy_index
+        _check_provenance(pr_per)
+        thr = threshold_in_units_of(thresh, pr) if isinstance(thresh, str) else float(thresh)
+        return bootstrap_doy_index(pr, pr_per, freq, op, (">", ">="), "sum", floor=thr)
     code = _lib.op_code(op, (">", ">="))
     thr = threshold_in_units_of(thresh, pr) if isinstance(thresh, str) else float(thresh)
     x2d, cell_shape, other, ta = _unwrap(pr)

@@ -290,14 +290,19 @@ class TimeAxis:
         starts = np.concatenate([[0], np.cumsum(out)[:-1]])
         return np.add.reduceat(keep, starts)
 
-    def bootstrap_group_ids(self, freq: str) -> np.ndarray:
+    @staticmethod
+    def bootstrap_freq(freq: str) -> str:
         """Year grouping used by the percentile bootstrap (core/bootstrapping.py:214-223):
         ``Y`` + ``S``/``E`` + the anchor of ``freq`` when its base is yearly or quarterly."""
         mult, base, start, anchor = parse_offset(freq)
         bfreq = "YS" if start else "YE"
         if base in ("Y", "Q") and anchor is not None:
             bfreq = f"{bfreq}-{anchor}"
-        return self.group_ids(bfreq)
+        return bfreq
+
+    def bootstrap_group_ids(self, freq: str) -> np.ndarray:
+        """Group ids of the bootstrap year grouping of ``freq`` (``bootstrap_freq``)."""
+        return self.group_ids(self.bootstrap_freq(freq))
 
     def date_index_in_periods(self, freq: str, date: str) -> np.ndarray:
         """Absolute index of the ``MM-DD`` date inside every ``resample(time=freq)`` group, -1 where the
