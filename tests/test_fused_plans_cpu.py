@@ -1,14 +1,14 @@
 """CPU checks of the fused multi-output pass around its kernel: the plan packer of ``indices.run_batch``
-(``_PassBuilder``), the condition normalisation, the restated dispatch of tests/multi_plan.py and the sequential
+(``_PassBuilder``), the condition normalisation, the launch plan of the entry point and the sequential
 oracle of oracle/multi_oracle.py against the reference-semantics compositions of oracle/xclim_oracle.py."""
 import numpy as np
 import pytest
 
 import fake_device
-from multi_plan import empty_plan, instantiations, multi_kernel, plan_errors
+from dispatch_host_build import multi_errors as plan_errors, multi_shape as multi_kernel
 from oracle import multi_oracle as MO
 from oracle import xclim_oracle as O
-from xb_helpers import make_field
+from xb_helpers import empty_plan, instantiations, make_field
 from xclim_b200 import _lib, device
 from xclim_b200.indices import _PassBuilder
 

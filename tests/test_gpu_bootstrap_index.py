@@ -40,6 +40,8 @@ def _bits(scratch, N, C):
                          ids=[f"N{c[0]}-W{c[1]}-p{c[2]:g}-{c[5]}-{c[6]}" for c in paths.CASES])
 def test_mask_popcount_equals_counts(cuda, monkeypatch, N, W, per, op, ab, kernel, layout):
     import torch
+    from dispatch_host_build import boot_plan
+    assert boot_plan(N, W, per, ab[0], ab[1], year_len=L, mask=True)[0] == kernel
     rng = np.random.default_rng(2000 + 37 * N + W + int(per))
     C = 161
     pre = 1 if layout == "offset" else 0

@@ -2,8 +2,8 @@
 
 The dispatch picks bootstrap5_kernel (window 5, <= 16 base years, <= 8 kept order statistics) or
 bootstrap_kernel<KA, KB> with 16x8, 32x16 or 32x32 kept values; above 32 base years every year takes the
-exact per-(y, s) loop.  Each case names the kernel it is meant to reach (tests/boot_dispatch.py restates
-the dispatch) and runs on short synthetic years (L = 40 days, so a tenth of the days are year-edge days and
+exact per-(y, s) loop.  Each case names the kernel it is meant to reach (the launch plan the launcher
+executes) and runs on short synthetic years (L = 40 days, so a tenth of the days are year-edge days and
 a day chunk ends inside the year) of hostile data: values on a 0.5 grid (ties, x equal to the threshold),
 signed zeros, NaN on edge days and whole NaN years, samples with fewer than two values, an all-NaN and a
 constant cell, +-inf at the interpolated ranks and finite +-3e38 whose neighbour difference overflows
@@ -12,7 +12,7 @@ float32.  Every count is compared bit for bit.
 import numpy as np
 import pytest
 
-from boot_dispatch import bootstrap_kernel, every_year_exact
+from dispatch_host_build import boot_kernel as bootstrap_kernel, exact_years as every_year_exact
 from oracle import xclim_oracle as O
 
 pytestmark = pytest.mark.gpu

@@ -1,17 +1,19 @@
 """The fused multi-output pass (`xc_period_multi_f32`, csrc/period_stats.cu) on hand-built plans, bit for bit
 against the sequential restatement of oracle/multi_oracle.py: every `period_multi_kernel<NC, NCR, NM, NS, VEC,
-UNROLL>` instantiation (named through the restated dispatch of tests/multi_plan.py), hostile data, grid edges and
+UNROLL>` instantiation (named through the launch plan the entry point executes), hostile data, grid edges and
 the plan checks; then `indices.run_batch` on the plan shapes and grids the default batch never builds."""
 import ctypes
 
 import numpy as np
 import pytest
 
-from multi_plan import empty_plan, instantiations, multi_kernel, plan_errors
+from dispatch_host_build import multi_errors as plan_errors, multi_shape as multi_kernel
 from oracle import multi_oracle as MO
+from xb_helpers import empty_plan, instantiations
 from xclim_b200 import _lib, device
 
 pytestmark = pytest.mark.gpu
+
 
 F32 = np.float32
 FMAX = float(np.finfo(F32).max)
@@ -295,7 +297,7 @@ def test_plan_rejections(case, cuda):
     mutate, msg = BAD_PLANS[case]
     x = torch.zeros((16, 8), device=cuda)
     plan = _bad(mutate)
-    assert plan_errors(plan, 5), "the restated checks accept it"
+    assert plan_errors(plan, 5), "the plan check accepts it"
     assert plan_errors(_ok_plan(), 5) == []
     _rejects(x.data_ptr(), 16, 8, 8, plan, 5, msg, cuda)
 

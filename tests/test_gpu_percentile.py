@@ -235,7 +235,7 @@ def test_percentile_doy_tma_path(cuda, years, per, monkeypatch):
     whose interpolation meets infinities or overflows (NaN lerp -> the sample maximum).  32 years take
     the 92nd / 8th percentile: the 90th / 10th need 17 order statistics there, beyond the TMA kernel's 16."""
     import torch
-    from pdoy_dispatch import kernels
+    from dispatch_host_build import pdoy_kernels as kernels
     from xclim_b200 import device
     rng = np.random.default_rng(100 + years)
     L, T = 365, years * 365

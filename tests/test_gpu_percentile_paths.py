@@ -3,7 +3,7 @@
 The dispatch picks, per percentile, the generic kernel (4..64 kept order statistics), the selection kernel,
 the ring kernel (uniform<8|16|32>), the paired window-5 kernel (w5p<8|16>) -- each of the last two on uniform
 years or through the (year, day-of-year) table -- or the TMA-fed window-5 kernel (w5t, 30..32 uniform years).
-Each case names the kernels it is meant to reach (tests/pdoy_dispatch.py restates the dispatch), checks that
+Each case names the kernels it is meant to reach (the launch plan the launcher executes), checks that
 name against the launches torch.profiler records, and compares the raw (n_per, n_doy, C) table with the
 oracle's table before its 365 -> 366 re-interpolation and with the generic kernel's.  The data hold scattered
 NaN, whole NaN years on some days, an all-NaN and a one-value cell, ties, signed zeros, and cells whose
@@ -17,10 +17,9 @@ import warnings
 import numpy as np
 import pytest
 
-from boot_dispatch import plan_quantile
+from dispatch_host_build import Unsupported, pdoy_plan as kernel_plan, quantile_plan as plan_quantile
 from oracle import xclim_oracle as O
-from pdoy_dispatch import Unsupported, kernel_plan, uniform_calendar
-from xb_helpers import plant_infinite_samples
+from xb_helpers import plant_infinite_samples, uniform_calendar
 
 pytestmark = pytest.mark.gpu
 
@@ -119,7 +118,7 @@ def _profiled(fn):
 
 
 def _check(xd, x_host, cal, window, pers, expect, sel=None, no_tma=False):
-    """Launches the restated plan names, the profiler's witness, the oracle's bits and the generic kernel's."""
+    """Launches the plan names, the profiler's witness, the oracle's bits and the generic kernel's."""
     import torch
     from xclim_b200 import device
     doy, year, ny, n_doy = _calendar(cal)

@@ -2,7 +2,7 @@
 and xc_spell_mask_f32 against the window-sum rule (oracle window_stat_rule: the float64 sum of the window in
 time order, NaN if any value is NaN, rounded once to float32).
 
-Each case names the kernel instances it is meant to reach (tests/rolling_dispatch.py restates the dispatch),
+Each case names the kernel instances it is meant to reach (the launch plans the launchers execute),
 checks them against the launches torch.profiler records, and compares the outputs with the rule: spell run
 statistics and rolling sum / min / max / count exactly, means, std and var at the tolerances of
 test_gpu_run_reducers.py.  Paths that see the same cells must agree: spell outputs bit for bit, rolling outputs by
@@ -18,7 +18,7 @@ import numpy as np
 import pytest
 
 from oracle import xclim_oracle as O
-import rolling_dispatch as D
+import dispatch_host_build as H
 
 pytestmark = pytest.mark.gpu
 
@@ -101,12 +101,12 @@ def _layout_args(v):
 
 def _spell_kernel(layout, w, ws, r, before):
     C, ldx, al = layout
-    return D.spell_kernel(C, ldx, w, ST[ws], RL[r], before, aligned_x=al)
+    return H.spell_instance(C, ldx, w, ST[ws], RL[r], before, aligned_x=al)
 
 
 def _rolling_kernel(layout, w, ws, s, center):
     C, ldx, al = layout
-    return D.rolling_kernel(C, ldx, w, ST[ws], ST[s], center, aligned_x=al)
+    return H.rolling_instance(C, ldx, w, ST[ws], ST[s], center, aligned_x=al)
 
 
 # ------------------------------------------------------------------------------------------------- launches
@@ -411,5 +411,5 @@ def hostile_sliding_instances():
     cells; test_spell_mask_season runs spell_mask at w = 7 and 12)."""
     out = {"spell_mask"}
     for w in WINDOWS:
-        out |= {k for k in _small_spell_instances(w) | _small_rolling_instances(w) if D.slides(k, w, ST["sum"])}
+        out |= {k for k in _small_spell_instances(w) | _small_rolling_instances(w) if H.instance_slides(k, w, ST["sum"])}
     return out

@@ -1,12 +1,14 @@
-"""The restated percentile_doy dispatch (tests/pdoy_dispatch.py) that the GPU path tests rely on to name the
-kernels each case runs, pinned on known plans: every template instance, the TMA eligibility, the shared-memory
-and selection caps, and table mode's day segmentation."""
+"""The percentile_doy launch plan (launch_plan.cuh, through the host build of tests/dispatch_host_build.py) that the
+GPU path tests rely on to name the kernels each case runs, pinned on known plans: every template instance, the TMA
+eligibility, the shared-memory and selection caps, table mode's day segmentation and the day splits."""
 import datetime
 
 import numpy as np
 import pytest
 
-from pdoy_dispatch import INSTANCES, Unsupported, kernel_plan, kernels, split_days, uniform_calendar
+from dispatch_host_build import PDOY_INSTANCES as INSTANCES, Unsupported
+from dispatch_host_build import pdoy_kernels as kernels, pdoy_plan as kernel_plan, split_plan as split_days
+from xb_helpers import uniform_calendar
 
 
 def _standard(start, end):
@@ -145,3 +147,17 @@ def test_percentile_offsets_in_one_call():
 ])
 def test_split_days(nd, cblocks, ctas, min_per, pairs, expect):
     assert split_days(nd, cblocks, ctas, min_per, pairs, sms=132) == expect
+
+
+@pytest.mark.parametrize("nd,cblocks,ctas,min_per,pairs,align,sms,expect", [
+    (365, 2, 12, 20, False, 32, 132, (12, 32)),      # whole mask words: 11 chunks of 32 days and one of 13
+    (365, 300, 6, 20, False, 32, 132, (3, 128)),     # 122 days rounded up to four words
+    (365, 10_000, 6, 20, False, 32, 132, (1, 365)),  # one chunk: the whole year
+    (40, 2, 12, 20, False, 32, 114, (2, 32)),        # the last chunk keeps the remaining 8 days
+    (365, 2, 16, 40, True, 32, 132, (6, 64)),        # whole pairs, then whole words
+    (30, 2, 6, 4, False, 32, 132, (1, 30)),          # a year shorter than one word: one chunk
+])
+def test_split_days_aligned(nd, cblocks, ctas, min_per, pairs, align, sms, expect):
+    chunks, per = split_days(nd, cblocks, ctas, min_per, pairs, sms=sms, align=align)
+    assert (chunks, per) == expect
+    assert per == nd or per % align == 0

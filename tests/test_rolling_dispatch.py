@@ -1,10 +1,16 @@
-"""CPU pin of tests/rolling_dispatch.py, the restated dispatch of the rolling-window and spell kernels
-(csrc/rolling.cu): a table naming every kernel instance the dispatch can pick, and the coverage of
+"""CPU pin of the rolling-window and spell launch plans (launch_plan.cuh, through the host build of
+tests/dispatch_host_build.py): a table naming every kernel instance the dispatch can pick, and the coverage of
 tests/test_gpu_rolling_paths.py measured against it."""
+import types
+
 import pytest
 
-import rolling_dispatch as D
-from rolling_dispatch import MAX, MEAN, MIN, SUM, Unsupported
+import dispatch_host_build as H
+from dispatch_host_build import MAX, MEAN, MIN, SUM, Unsupported
+
+D = types.SimpleNamespace(spell_kernel=H.spell_instance, rolling_kernel=H.rolling_instance, slides=H.instance_slides,
+                          can_stream4=H.can_stream4, INSTANCES=H.INSTANCES, SPELL_SUMW=H.SPELL_SUMW,
+                          ROLLING_SUMW=H.ROLLING_SUMW, SLIDING=H.SLIDING)
 
 RL = {"max": 0, "min": 1, "sum": 2, "count": 3, "mean": 4, "std": 5}
 STAT = {"sum": 0, "mean": 1, "min": 2, "max": 3, "std": 4, "var": 5, "count": 6}

@@ -13,6 +13,39 @@ def make_field(values, start="2000-01-01", calendar="standard", units="K", dims=
     return Field(values, dims, ta, {}, {"units": units, **attrs})
 
 
+def uniform_calendar(L, n_years):
+    """(doy, year) of ``n_years`` whole years of ``L`` days."""
+    t = np.arange(L * n_years)
+    return t % L + 1, t // L
+
+
+def instantiations():
+    """The 38 instantiated (NC, NCR, NM, NS) of period_multi_kernel."""
+    out = [(0, 0, 0, 0), (0, 0, 0, 3)]
+    for nc in (2, 4, 6):
+        for nm in (0, 1):
+            for ncr in (0, 1, 2):
+                for ns in (0, 3):
+                    out.append((nc, ncr, nm, ns))
+    return out
+
+
+def empty_plan():
+    """A fused-pass plan with no outputs: every slot -1, every entry at its neutral value."""
+    from xclim_b200 import _lib
+    plan = _lib.MultiPlan()
+    plan.slot_sum = plan.slot_mean = plan.slot_min = plan.slot_max = -1
+    for j in range(_lib.MULTI_MAX_COND):
+        plan.cond[j].slot_n = plan.cond[j].slot_max = -1
+        plan.cond[j].wmax = 1
+    for k in range(_lib.MULTI_MAX_RUNS):
+        plan.runs[k].cond, plan.runs[k].window, plan.runs[k].slot = k // 2, 1, -1
+    plan.msum[0].slot, plan.msum[0].window = -1, 1
+    for k in range(_lib.MULTI_MAX_SUMS):
+        plan.sums[k].slot = -1
+    return plan
+
+
 def plant_infinite_samples(x, qs, cells, seed=0):
     """Overwrite five cells per quantile q of ``x`` (time first; ``cells`` are flat cell indexes, used in
     order) with infinite or overflowing values placed around the q-quantile's neighbours, so that the

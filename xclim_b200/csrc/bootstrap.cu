@@ -28,13 +28,12 @@
 
 #include "bootstrap_reduce_core.cuh"
 #include "common.cuh"
+#include "launch_plan.cuh"
 #include "quantile.cuh"
 #include "sortnet.cuh"
 
 namespace xc {
 namespace {
-
-constexpr int kThreads = 128;
 
 // output of the exceedance kernels: per-period counts (tx90p & family) or per-(y, s) day masks
 constexpr int kCount = 0, kMask = 1;
@@ -251,7 +250,7 @@ bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t ba
       const int k1min = top ? (na - 2 - q0.ilo) : q0.ilo;
       const int k1max = top ? (na + W - 2 - q1.ilo) : q1.ilo;
       bool decided = false;
-      if (ok0 && ok1 && N <= 32 && !hostile) {
+      if (ok0 && ok1 && N <= kBootExactAbove && !hostile) {
         if (gtA >= k1max + 2) {
           decided = true;                       // never beats the threshold
         } else if (geT < KA && geA + W <= k1min) {
@@ -260,13 +259,13 @@ bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t ba
           else set_year_bits<OP>(mo, C, c, N, y, d, (double)xq);
         }
       }
-      if (!decided) band |= (N <= 32) ? (1u << y) : 0u;
+      if (!decided) band |= (N <= kBootExactAbove) ? (1u << y) : 0u;
     }
-    // exact evaluation of the in-band years (all years when N > 32)
+    // exact evaluation of the in-band years (all years when N > kBootExactAbove)
     int y_all = 0;
     while (true) {
       int y = -1;
-      if (N <= 32) {
+      if (N <= kBootExactAbove) {
         if (band) { y = __ffs(band) - 1; band &= band - 1u; }
       } else if (y_all < N) {
         y = y_all++;
@@ -353,7 +352,6 @@ bootstrap_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t ba
 // (544 bytes for N = 15: the sorted day lists are rebuilt from the raw ring instead of being kept, which
 // trades 7 % more instructions for 50 % more resident warps in a latency-bound kernel).  N <= 16.
 // ------------------------------------------------------------------------------------------------
-constexpr int kBT = 32;   // threads per CTA: one warp
 constexpr float kPosInf = __builtin_huge_valf();
 
 __device__ __forceinline__ void sort5_desc(float& a, float& b, float& c, float& d, float& e) {
@@ -685,28 +683,6 @@ bootstrap5_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int64_t b
   }
 }
 
-template <int MODE>
-int32_t launch_bootstrap5(int32_t op, const float* x, int64_t C, int64_t ldx, int64_t base_start, int32_t N, int32_t L,
-                          const QuantSpec& spec, const int32_t* step_period, int32_t* counts, const MaskOut& mo,
-                          cudaStream_t st) {
-  const int64_t cblocks = (C + kBT - 1) / kBT;
-  const DaySplit sp = split_days(L, cblocks, 12, 20, false, MODE == kMask ? 32 : 1);
-  const size_t smem = ((size_t)8 * N + 16) * kBT * 4;
-  if (smem > 227 * 1024) return 1;
-  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
-  return dispatch_op(op, [&](auto OPC) -> int32_t {
-    constexpr int OP = decltype(OPC)::value;
-    if (smem > 48 * 1024) {
-      cudaError_t e = cudaFuncSetAttribute(bootstrap5_kernel<OP, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)smem);
-      if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(bootstrap5_kernel)");
-    }
-    bootstrap5_kernel<OP, MODE><<<grid, kBT, smem, st>>>(x, C, ldx, base_start, N, L, spec, step_period, sp.per,
-                                                         counts, mo);
-    return launch_status("bootstrap5_kernel");
-  });
-}
-
 __global__ void __launch_bounds__(256)
 bootstrap_finish_kernel(const int32_t* __restrict__ counts, int64_t n, double denom, double* __restrict__ out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -714,53 +690,41 @@ bootstrap_finish_kernel(const int32_t* __restrict__ counts, int64_t n, double de
 }
 
 template <int KA, int KB, int MODE>
-int32_t launch_bootstrap(int32_t op, const float* x, int64_t C, int64_t ldx, int64_t base_start, int32_t N,
-                         int32_t L, int32_t W, const QuantSpec& spec, const int32_t* step_period, int32_t* counts,
+int32_t launch_bootstrap(const BootPlan& p, int32_t op, const float* x, int64_t C, int64_t ldx, int64_t base_start,
+                         int32_t N, int32_t L, int32_t W, const int32_t* step_period, int32_t* counts,
                          const MaskOut& mo, cudaStream_t st) {
-  const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  const DaySplit sp = split_days(L, cblocks, 6, 4 * W, false, MODE == kMask ? 32 : 1);
-  const size_t smem = ((size_t)(W - 1) * (KA + 1) + (size_t)W * N) * kThreads * 4;
-  if (smem > 227 * 1024) {
-    set_error("bootstrap: %d base years x window %d need %zu bytes of shared memory per block", N, W, smem);
-    return XC_ERR_UNSUPPORTED;
-  }
-  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
   return dispatch_op(op, [&](auto OPC) -> int32_t {
-    constexpr int OP = decltype(OPC)::value;
-    if (smem > 48 * 1024) {
-      cudaError_t e = cudaFuncSetAttribute(bootstrap_kernel<KA, KB, OP, MODE>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(bootstrap_kernel)");
-    }
-    bootstrap_kernel<KA, KB, OP, MODE><<<grid, kThreads, smem, st>>>(x, C, ldx, base_start, N, L, W, spec,
-                                                                     step_period, sp.per, counts, mo);
+    auto kern = bootstrap_kernel<KA, KB, decltype(OPC)::value, MODE>;
+    if (int32_t e = allow_smem(kern, p.smem, "cudaFuncSetAttribute(bootstrap_kernel)")) return e;
+    kern<<<dim3((unsigned)p.cblocks, (unsigned)p.split.chunks, 1), kThreads, p.smem, st>>>(
+        x, C, ldx, base_start, N, L, W, p.spec, step_period, p.split.per, counts, mo);
     return launch_status("bootstrap_kernel");
   });
 }
 
-// The exceedance kernel for `need` order statistics of the window-W sample: the same choice in both modes
+// The exceedance kernel of plan_bootstrap: the same choice in both modes
 template <int MODE>
 int32_t launch_exceedance(const float* x, int64_t C, int64_t ldx, int64_t base_start, int32_t N, int32_t L,
                           int32_t window, double percentile, double alpha, double beta, int32_t op,
                           const int32_t* step_period, int32_t* counts, const MaskOut& mo, cudaStream_t st) {
-  QuantSpec spec;
-  const int need = plan_quantile(percentile, alpha, beta, N * window, &spec);
-  int32_t e = 1;
-  if (need > 0 && need <= 8 && window == 5 && N <= 16 && L > 8 && !getenv("XCLIM_B200_BOOT_V1"))
-    e = launch_bootstrap5<MODE>(op, x, C, ldx, base_start, N, L, spec, step_period, counts, mo, st);
-  if (e != 1) {
-  } else if (need > 0 && need <= 8 && need + window <= 16)
-    e = launch_bootstrap<16, 8, MODE>(op, x, C, ldx, base_start, N, L, window, spec, step_period, counts, mo, st);
-  else if (need > 0 && need <= 16 && need + window <= 32)
-    e = launch_bootstrap<32, 16, MODE>(op, x, C, ldx, base_start, N, L, window, spec, step_period, counts, mo, st);
-  else if (need > 0 && need + window <= 32)
-    e = launch_bootstrap<32, 32, MODE>(op, x, C, ldx, base_start, N, L, window, spec, step_period, counts, mo, st);
-  else {
-    set_error("bootstrap: percentile %g of %d samples needs %d order statistics (+%d removals); at most 32 are kept",
-              percentile, N * window, need, window);
-    return XC_ERR_UNSUPPORTED;
-  }
-  return e;
+  BootPlan p;
+  const int32_t ep = plan_bootstrap(N, L, window, percentile, alpha, beta, MODE == kMask,
+                                    getenv("XCLIM_B200_BOOT_V1") != nullptr, C, sm_count(), &p);
+  if (ep) return ep;
+  if (p.kernel == kBoot5)
+    return dispatch_op(op, [&](auto OPC) -> int32_t {
+      auto kern = bootstrap5_kernel<decltype(OPC)::value, MODE>;
+      if (int32_t e = allow_smem(kern, p.smem, "cudaFuncSetAttribute(bootstrap5_kernel)")) return e;
+      kern<<<dim3((unsigned)p.cblocks, (unsigned)p.split.chunks, 1), kBT, p.smem, st>>>(
+          x, C, ldx, base_start, N, L, p.spec, step_period, p.split.per, counts, mo);
+      return launch_status("bootstrap5_kernel");
+    });
+#define XC_BOOT(E) launch_bootstrap<kBoot[E].ka, kBoot[E].kb, MODE>(p, op, x, C, ldx, base_start, N, L, window, \
+                                                                  step_period, counts, mo, st)
+  if (p.kernel == kBoot16x8) return XC_BOOT(kBoot16x8);
+  if (p.kernel == kBoot32x16) return XC_BOOT(kBoot32x16);
+  return XC_BOOT(kBoot32x32);
+#undef XC_BOOT
 }
 
 // One lane per (cell, in-base year y = blockIdx.y): year y's index against each altered table, averaged

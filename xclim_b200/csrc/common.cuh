@@ -226,24 +226,6 @@ inline int sm_count() {
   return n;
 }
 
-// Day split of the day-of-year kernels: blockIdx.y walks `chunks` chunks of `per` consecutive days.  Enough
-// chunks that the cblocks cell blocks give ctas_per_sm CTAs per SM, but at least min_per days per chunk (each
-// chunk pays a halo of extra days), rounded up to whole pairs of days when `pairs` and to a multiple of `align`
-// days (every chunk starts on a multiple of `align`).
-struct DaySplit {
-  int chunks, per;
-};
-inline DaySplit split_days(int nd, int64_t cblocks, int ctas_per_sm, int min_per, bool pairs, int align = 1) {
-  int chunks = (int)((sm_count() * ctas_per_sm + cblocks - 1) / cblocks);
-  if (chunks < 1) chunks = 1;
-  int per = (nd + chunks - 1) / chunks;
-  if (per < min_per) per = min_per;
-  if (pairs) per = (per + 1) & ~1;
-  per = (per + align - 1) / align * align;
-  if (per > nd) per = nd;
-  return {(nd + per - 1) / per, per};
-}
-
 // Time split of the streaming quantile-mapping kernels: blockIdx.y walks `chunks` chunks of `rows` steps.  Enough
 // chunks for 16 CTAs per SM over the cblocks cell blocks, each at least min_rows steps, rounded up to whole `align`s.
 struct RowSplit {

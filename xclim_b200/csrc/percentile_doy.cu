@@ -27,13 +27,12 @@
 #include <vector>
 
 #include "common.cuh"
+#include "launch_plan.cuh"
 #include "quantile.cuh"
 #include "sortnet.cuh"
 
 namespace xc {
 namespace {
-
-constexpr int kThreads = 128;
 
 __device__ __forceinline__ void store_vec4(int32_t* dst, const int32_t (&v)[4]) {
   *reinterpret_cast<int4*>(dst) = make_int4(v[0], v[1], v[2], v[3]);
@@ -133,8 +132,6 @@ percentile_doy_generic_kernel(const float* __restrict__ x, int64_t T, int64_t C,
 // smallest key above it unless ties already cover rank k+1.  Exact for any sample that fits shared
 // memory (n_years * window <= 768); ~30x the cost of the network kernels, used only when needed.
 // ------------------------------------------------------------------------------------------------
-constexpr int kSelThreads = 64;
-
 __device__ __forceinline__ uint32_t order_key(float v) {
   const uint32_t b = __float_as_uint(v);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
@@ -619,8 +616,7 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
       : "memory");
 }
 
-constexpr int kTmaCells = kThreads;                 // cells per CTA = consumer threads
-constexpr int kTmaThreads = kThreads + 32;          // + one producer warp
+constexpr int kTmaThreads = kTmaCells + 32;         // one consumer thread per cell + one producer warp
 
 template <int N2>   // years = 16 + N2, N2 in {14, 15, 16}
 __global__ void __launch_bounds__(kTmaThreads, 3)
@@ -882,100 +878,8 @@ doy_count_years_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, int6
   }
 }
 
-// generic kernel with the shortest list that holds `need` (<= 64) order statistics
-int32_t launch_generic(int need, const float* x, int64_t T, int64_t C, int64_t ldx, const int32_t* pos, int32_t n_doy,
-                       int32_t n_years, int32_t h, const QuantSpec& spec, double* out, cudaStream_t st,
-                       int d_begin = 0, int d_end = -1, const int32_t* vrow = nullptr) {
-  if (d_end < 0) d_end = n_doy;
-  const int nd = d_end - d_begin;
-  if (nd <= 0) return XC_OK;
-  const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  const DaySplit sp = split_days(nd, cblocks, 8, 1, false);
-  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
-  auto go = [&](auto kern) -> int32_t {
-    kern<<<grid, kThreads, 0, st>>>(x, T, C, ldx, pos, n_doy, n_years, h, spec, sp.per, out, d_begin, d_end, vrow);
-    return launch_status("percentile_doy_generic_kernel");
-  };
-  if (need <= 4) return go(percentile_doy_generic_kernel<4>);
-  if (need <= 8) return go(percentile_doy_generic_kernel<8>);
-  if (need <= 16) return go(percentile_doy_generic_kernel<16>);
-  if (need <= 32) return go(percentile_doy_generic_kernel<32>);
-  return go(percentile_doy_generic_kernel<64>);
-}
-
-// pos == nullptr: uniform years (days [0, L)); else table mode on the interior days [d_begin, d_end)
-template <int K>
-int32_t launch_uniform(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t L, int32_t N, int32_t W,
-                       const QuantSpec& spec, double* out, cudaStream_t st, const int32_t* pos = nullptr,
-                       int n_doy = 0, int d_begin = 0, int d_end = -1) {
-  if (d_end < 0) d_end = L;
-  const int nd = d_end - d_begin;
-  if (nd <= 0) return XC_OK;
-  const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  // at least 8 W days per chunk keeps the halo overhead (W-1 extra day lists per chunk) small
-  const DaySplit sp = split_days(nd, cblocks, 12, 8 * W, false);
-  const size_t smem = (size_t)(W - 1) * (K + 1) * kThreads * 4;
-  if (smem > 48 * 1024) {
-    cudaError_t e = pos ? cudaFuncSetAttribute(percentile_doy_uniform_kernel<K, true>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                        : cudaFuncSetAttribute(percentile_doy_uniform_kernel<K, false>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(percentile_doy_uniform_kernel)");
-  }
-  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
-  if (pos)
-    percentile_doy_uniform_kernel<K, true><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, W, spec, sp.per,
-                                                                         out, pos, n_doy, d_begin, d_end);
-  else
-    percentile_doy_uniform_kernel<K, false><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, W, spec, sp.per,
-                                                                          out, pos, n_doy, d_begin, d_end);
-  return launch_status("percentile_doy_uniform_kernel");
-}
-
-template <int K>
-int32_t launch_w5(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t L, int32_t N, const QuantSpec& spec,
-                  double* out, cudaStream_t st, const int32_t* pos = nullptr, int n_doy = 0, int d_begin = 0,
-                  int d_end = -1) {
-  if (d_end < 0) d_end = L;
-  const int nd = d_end - d_begin;
-  if (nd <= 0) return XC_OK;
-  const int64_t cblocks = (C + kThreads - 1) / kThreads;
-  const DaySplit sp = split_days(nd, cblocks, 16, 40, true);   // 4 extra day lists per chunk, whole pairs of days
-  // 4 lists + 4 counts per lane, plus the 32-row staging column of the cp.async prefetch
-  const size_t smem = (size_t)4 * (K + 1) * kThreads * 4 + (K == 16 && !pos ? (size_t)32 * kThreads * 4 : 0);
-  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
-  if (smem > 48 * 1024) {
-    cudaError_t e = pos ? cudaFuncSetAttribute(percentile_doy_w5p_kernel<K, true>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                        : cudaFuncSetAttribute(percentile_doy_w5p_kernel<K, false>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(percentile_doy_w5p_kernel)");
-  }
-  if (pos)
-    percentile_doy_w5p_kernel<K, true><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, spec, sp.per, out,
-                                                                     pos, n_doy, d_begin, d_end);
-  else
-    percentile_doy_w5p_kernel<K, false><<<grid, kThreads, smem, st>>>(x, (int32_t)T, C, ldx, L, N, spec, sp.per, out,
-                                                                      pos, n_doy, d_begin, d_end);
-  return launch_status("percentile_doy_w5p_kernel");
-}
-
-// Day-list kernel for `need` (<= 32) order statistics and window `W`: the paired kernel for window 5 and
-// need <= 16, else the ring kernel.  pos == nullptr: uniform years; else table mode on [d_begin, d_end).
-int32_t launch_day_lists(int need, int32_t W, const float* x, int64_t T, int64_t C, int64_t ldx, int32_t L, int32_t N,
-                         const QuantSpec& spec, double* out, cudaStream_t st, const int32_t* pos = nullptr,
-                         int n_doy = 0, int d_begin = 0, int d_end = -1) {
-  if (W == 5 && need <= 16)
-    return need <= 8 ? launch_w5<8>(x, T, C, ldx, L, N, spec, out, st, pos, n_doy, d_begin, d_end)
-                     : launch_w5<16>(x, T, C, ldx, L, N, spec, out, st, pos, n_doy, d_begin, d_end);
-  if (need <= 8) return launch_uniform<8>(x, T, C, ldx, L, N, W, spec, out, st, pos, n_doy, d_begin, d_end);
-  if (need <= 16) return launch_uniform<16>(x, T, C, ldx, L, N, W, spec, out, st, pos, n_doy, d_begin, d_end);
-  return launch_uniform<32>(x, T, C, ldx, L, N, W, spec, out, st, pos, n_doy, d_begin, d_end);
-}
-
-
-// TMA path of launch_w5<16>: needs a 16-byte aligned base, ldx % 4 == 0 (global strides are multiples of
-// 16 bytes) and 30..32 years.  Returns 1 when the shape does not qualify (caller falls back).
+// The TMA kernel's view of x: boxes of kTmaCells cells x 1 day x N years.  The driver's encoder is fetched at run
+// time; false when it is missing or rejects the map.
 typedef CUresult (*XcEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -993,34 +897,90 @@ static XcEncodeTiled tensor_map_encoder() {
   return fn;
 }
 
-int32_t launch_w5_tma(const float* x, int64_t T, int64_t C, int64_t ldx, int32_t L, int32_t N, const QuantSpec& spec,
-                      double* out, cudaStream_t st) {
-  if (N < 30 || N > 32 || (ldx % 4) != 0 || !aligned16(x) || T != (int64_t)L * N || L < 8) return 1;
-  if (C > 2147483647LL - kTmaCells) return 1;
+bool encode_w5t_map(CUtensorMap* map, const float* x, int64_t C, int64_t ldx, int32_t L, int32_t N) {
   XcEncodeTiled enc = tensor_map_encoder();
-  if (!enc) return 1;
-  CUtensorMap map;
+  if (!enc) return false;
   const cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)L, (cuuint64_t)N};
   const cuuint64_t strides[2] = {(cuuint64_t)ldx * 4ull, (cuuint64_t)L * (cuuint64_t)ldx * 4ull};
   const cuuint32_t box[3] = {(cuuint32_t)kTmaCells, 1u, (cuuint32_t)N};
   const cuuint32_t estr[3] = {1u, 1u, 1u};
-  const CUresult r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NAN_REQUEST_ZERO_FMA);
-  if (r != CUDA_SUCCESS) return 1;
-  const int64_t cblocks = (C + kTmaCells - 1) / kTmaCells;
-  const DaySplit sp = split_days(L, cblocks, 12, 40, true);   // 4 extra day lists per chunk, whole pairs of days
-  const size_t smem = (size_t)2 * N * kTmaCells * 4 + (size_t)4 * (16 + 1) * kThreads * 4 + 64;
-  dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
-  auto go = [&](auto kern) -> int32_t {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(percentile_doy_w5t_kernel)");
-    kern<<<grid, kTmaThreads, smem, st>>>(map, C, L, spec, sp.per, out, 0, L, x, ldx);
+  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, estr,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NAN_REQUEST_ZERO_FMA) == CUDA_SUCCESS;
+}
+
+// One launch of the plan into `out` (its percentile's table).  pos / posrow / vrow: the uploaded (year, doy) -> step
+// table, the same table through the virtual-row map, and the map (null where the plan reads none of them).
+int32_t launch_pdoy(const PdoyLaunch& ln, const float* x, int64_t T, int64_t C, int64_t ldx, int32_t n_doy,
+                    int32_t n_years, int32_t window, const int32_t* pos, const int32_t* posrow, const int32_t* vrow,
+                    double* out, int sms, cudaStream_t st) {
+  const dim3 grid((unsigned)ln.cblocks, (unsigned)ln.chunks, 1);
+  const QuantSpec& spec = ln.spec;
+  const bool table = kPdoy[ln.kernel].table;
+  const int32_t* lists_pos = table ? posrow : nullptr;
+  const int32_t lists_n_doy = table ? n_doy : 0;
+  auto generic = [&](auto kern) -> int32_t {
+    kern<<<grid, kThreads, 0, st>>>(x, T, C, ldx, pos, n_doy, n_years, window / 2, spec, ln.per, out, ln.a, ln.b,
+                                    vrow);
+    return launch_status("percentile_doy_generic_kernel");
+  };
+  auto uniform = [&](auto kern) -> int32_t {
+    if (int32_t e = allow_smem(kern, ln.smem, "cudaFuncSetAttribute(percentile_doy_uniform_kernel)")) return e;
+    kern<<<grid, kThreads, ln.smem, st>>>(x, (int32_t)T, C, ldx, n_doy, n_years, window, spec, ln.per, out, lists_pos,
+                                          lists_n_doy, ln.a, ln.b);
+    return launch_status("percentile_doy_uniform_kernel");
+  };
+  auto w5p = [&](auto kern) -> int32_t {
+    if (int32_t e = allow_smem(kern, ln.smem, "cudaFuncSetAttribute(percentile_doy_w5p_kernel)")) return e;
+    kern<<<grid, kThreads, ln.smem, st>>>(x, (int32_t)T, C, ldx, n_doy, n_years, spec, ln.per, out, lists_pos,
+                                          lists_n_doy, ln.a, ln.b);
+    return launch_status("percentile_doy_w5p_kernel");
+  };
+  auto w5t = [&](auto kern) -> int32_t {
+    CUtensorMap map;
+    if (!encode_w5t_map(&map, x, C, ldx, n_doy, n_years)) {
+      // the one choice the plan cannot make: without the driver's encoder the same days go to w5p<16, false>
+      PdoyLaunch lanes = pdoy_day_lists(16, 5, ln.ip, ln.a, ln.b, C, false, sms);
+      lanes.spec = spec;
+      return launch_pdoy(lanes, x, T, C, ldx, n_doy, n_years, window, pos, posrow, vrow, out, sms, st);
+    }
+    if (int32_t e = allow_smem(kern, ln.smem, "cudaFuncSetAttribute(percentile_doy_w5t_kernel)")) return e;
+    kern<<<grid, kTmaThreads, ln.smem, st>>>(map, C, n_doy, spec, ln.per, out, ln.a, ln.b, x, ldx);
     return launch_status("percentile_doy_w5t_kernel");
   };
-  if (N == 30) return go(percentile_doy_w5t_kernel<14>);
-  if (N == 31) return go(percentile_doy_w5t_kernel<15>);
-  return go(percentile_doy_w5t_kernel<16>);
+  switch (ln.kernel) {
+#define XC_K(E) kPdoy[E].k
+#define XC_KT(E) kPdoy[E].k, kPdoy[E].table
+    case kGeneric4: return generic(percentile_doy_generic_kernel<XC_K(kGeneric4)>);
+    case kGeneric8: return generic(percentile_doy_generic_kernel<XC_K(kGeneric8)>);
+    case kGeneric16: return generic(percentile_doy_generic_kernel<XC_K(kGeneric16)>);
+    case kGeneric32: return generic(percentile_doy_generic_kernel<XC_K(kGeneric32)>);
+    case kGeneric64: return generic(percentile_doy_generic_kernel<XC_K(kGeneric64)>);
+    case kSelect: {
+      const size_t smem = ln.smem;
+      if (smem > 48 * 1024)
+        XC_CHECK_CUDA(cudaFuncSetAttribute(percentile_doy_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)smem));
+      percentile_doy_select_kernel<<<grid, kSelThreads, smem, st>>>(x, T, C, ldx, pos, n_doy, n_years, window / 2,
+                                                                    spec, ln.per, out, vrow);
+      return launch_status("percentile_doy_select_kernel");
+    }
+    case kW5t14: return w5t(percentile_doy_w5t_kernel<XC_K(kW5t14)>);
+    case kW5t15: return w5t(percentile_doy_w5t_kernel<XC_K(kW5t15)>);
+    case kW5t16: return w5t(percentile_doy_w5t_kernel<XC_K(kW5t16)>);
+    case kW5p8T: return w5p(percentile_doy_w5p_kernel<XC_KT(kW5p8T)>);
+    case kW5p8: return w5p(percentile_doy_w5p_kernel<XC_KT(kW5p8)>);
+    case kW5p16T: return w5p(percentile_doy_w5p_kernel<XC_KT(kW5p16T)>);
+    case kW5p16: return w5p(percentile_doy_w5p_kernel<XC_KT(kW5p16)>);
+    case kUniform8T: return uniform(percentile_doy_uniform_kernel<XC_KT(kUniform8T)>);
+    case kUniform8: return uniform(percentile_doy_uniform_kernel<XC_KT(kUniform8)>);
+    case kUniform16T: return uniform(percentile_doy_uniform_kernel<XC_KT(kUniform16T)>);
+    case kUniform16: return uniform(percentile_doy_uniform_kernel<XC_KT(kUniform16)>);
+    case kUniform32T: return uniform(percentile_doy_uniform_kernel<XC_KT(kUniform32T)>);
+    default: return uniform(percentile_doy_uniform_kernel<XC_KT(kUniform32)>);
+#undef XC_KT
+#undef XC_K
+  }
 }
 
 }  // namespace
@@ -1035,19 +995,6 @@ extern "C" int64_t xc_percentile_doy_workspace_bytes(int64_t T, int64_t C, int32
   return 2 * (int64_t)n_doy * (int64_t)n_years * 4 + T * 4 + 256;
 }
 
-// (year, doy) -> step table: pos[y * n_doy + d - 1] = the step of day-of-year d of year y, -1 where there is
-// none.  Returns the first step whose indexes are out of range, or -1.
-static int64_t build_pos_table(int64_t T, const int16_t* doy_index_host, const int16_t* year_index_host,
-                               int32_t n_doy, int32_t n_years, std::vector<int32_t>& pos) {
-  pos.assign((size_t)n_doy * n_years, -1);
-  for (int64_t t = 0; t < T; ++t) {
-    const int d = doy_index_host[t], y = year_index_host[t];
-    if (d < 1 || d > n_doy || y < 0 || y >= n_years) return t;
-    pos[(size_t)y * n_doy + (d - 1)] = (int32_t)t;
-  }
-  return -1;
-}
-
 static int32_t percentile_doy_impl(const float* x, int64_t T, int64_t C, int64_t ldx,
                                    const int16_t* doy_index_host, const int16_t* year_index_host,
                                    int32_t n_doy, int32_t n_years, int32_t window,
@@ -1058,34 +1005,30 @@ static int32_t percentile_doy_impl(const float* x, int64_t T, int64_t C, int64_t
   XC_REQUIRE(T > 0 && C > 0 && ldx >= C && T < 2147483647LL, "bad shape");
   XC_REQUIRE(n_doy > 0 && n_doy <= 366 && n_years > 0 && n_per > 0, "bad calendar description");
   XC_REQUIRE(window >= 1, "window must be >= 1");
-  if (window % 2 == 0) {
-    set_error("even `window` (xarray's center=True convention for even windows) is not supported");
-    return XC_ERR_UNSUPPORTED;
-  }
-  const int h = window / 2;
+  const int sms = sm_count();
+  PdoyPlan plan;
+  const int32_t ep = plan_percentile_doy(T, doy_index_host, year_index_host, vrow_host != nullptr, n_doy, n_years,
+                                         window, percentiles_host, n_per, alpha, beta, C, ldx, aligned16(x),
+                                         getenv("XCLIM_B200_NO_TMA") != nullptr, sms, &plan);
+  if (ep) return ep;
   cudaStream_t st = (cudaStream_t)stream;
 
-  std::vector<int32_t> pos;
-  const int64_t bad = build_pos_table(T, doy_index_host, year_index_host, n_doy, n_years, pos);
-  XC_REQUIRE(bad < 0, "doy/year index out of range at step %lld", (long long)bad);
-  // uniform-year fast path: step t is day t % n_doy of year t / n_doy
-  bool uniform = !vrow_host && T == (int64_t)pos.size();
-  for (size_t k = 0; uniform && k < pos.size(); ++k) uniform = (pos[k] == (int32_t)k);
-
+  // The tables go to the workspace only when a launch reads them, so a uniform calendar served by the day-list
+  // kernels needs no workspace.
+  const std::vector<int32_t>& pos = plan.pos;
   int32_t* pos_d = nullptr;      // (year, doy) -> step
   int32_t* posrow_d = nullptr;   // (year, doy) -> row holding that step's value (== pos_d without vrow)
   int32_t* vrow_d = nullptr;     // step -> row
-  // The tables go to the workspace when the first kernel that reads them is launched, so a uniform
-  // calendar served by the day-list kernels needs no workspace.
-  auto upload_tables = [&]() -> int32_t {
-    if (pos_d) return XC_OK;
+  bool tables = false;
+  for (const PdoyLaunch& ln : plan.launches) tables = tables || kPdoy[ln.kernel].table;
+  std::vector<int32_t> posrow;
+  if (tables) {
     const int64_t nb = (int64_t)pos.size() * 4;
     const int64_t need = vrow_host ? 2 * nb + T * 4 : nb;
     XC_REQUIRE(workspace != nullptr && workspace_bytes >= need, "workspace too small: need %lld bytes", (long long)need);
     pos_d = (int32_t*)workspace;
     posrow_d = pos_d;
     XC_CHECK_CUDA(cudaMemcpyAsync(pos_d, pos.data(), (size_t)nb, cudaMemcpyHostToDevice, st));
-    std::vector<int32_t> posrow;
     if (vrow_host) {
       for (int64_t t = 0; t < T; ++t)
         XC_REQUIRE(vrow_host[t] >= -1 && vrow_host[t] < T, "virtual row out of range at step %lld", (long long)t);
@@ -1098,86 +1041,10 @@ static int32_t percentile_doy_impl(const float* x, int64_t T, int64_t C, int64_t
     }
     // the tables live on this stack frame: make sure the copies have been issued from pageable memory
     XC_CHECK_CUDA(cudaStreamSynchronize(st));
-    return XC_OK;
-  };
-  // every kernel reads them when the years differ: check the workspace (and vrow) before anything else
-  if (!uniform) {
-    const int32_t e = upload_tables();
-    if (e) return e;
   }
-
-  // interior days whose windows never leave the year: [h, L_int - h) with L_int the shortest full year
-  const int L_int = (n_doy == 366) ? 365 : n_doy;
-  for (int ip = 0; ip < n_per; ++ip) {
-    const double per = percentiles_host[ip];
-    XC_REQUIRE(per >= 0.0 && per <= 100.0, "percentiles must be in [0, 100], got %g", per);
-    QuantSpec spec;
-    const int need = plan_quantile(per, alpha, beta, n_years * window, &spec);
-    if (need < 0) {
-      set_error("percentile %g with alpha=%g beta=%g: plotting positions outside [0, 1] are not supported", per,
-                alpha, beta);
-      return XC_ERR_UNSUPPORTED;
-    }
-    double* o = out + (int64_t)ip * n_doy * C;
-    if (need > 64) {
-      // order statistics far from both ends of the sample (e.g. the median): selection kernel
-      const int nmax = n_years * window;
-      if (nmax > 768) {
-        set_error("percentile %g of up to %d samples: the selection kernel holds at most 768 samples per cell", per,
-                  nmax);
-        return XC_ERR_UNSUPPORTED;
-      }
-      const int32_t eu = upload_tables();
-      if (eu) return eu;
-      const size_t smem = (size_t)nmax * kSelThreads * 4;
-      if (smem > 48 * 1024)
-        XC_CHECK_CUDA(cudaFuncSetAttribute(percentile_doy_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)smem));
-      const int64_t cblocks = (C + kSelThreads - 1) / kSelThreads;
-      const DaySplit sp = split_days(n_doy, cblocks, 8, 1, false);
-      dim3 grid((unsigned)cblocks, (unsigned)sp.chunks, 1);
-      percentile_doy_select_kernel<<<grid, kSelThreads, smem, st>>>(x, T, C, ldx, pos_d, n_doy, n_years, h, spec,
-                                                                    sp.per, o, vrow_d);
-      const int32_t es = launch_status("percentile_doy_select_kernel");
-      if (es) return es;
-      continue;
-    }
-    const int kk = need <= 8 ? 8 : need <= 16 ? 16 : 32;
-    const size_t smem_need = (size_t)(window - 1) * (kk + 1) * kThreads * 4;
-    const bool fast_ok = window >= 3 && need <= 32 && smem_need <= 200 * 1024 && (L_int - 2 * h) >= 8;
-    int32_t e = XC_OK;
-    if (uniform && fast_ok) {
-      e = 1;
-      if (window == 5 && need > 8 && need <= 16 && !getenv("XCLIM_B200_NO_TMA"))
-        e = launch_w5_tma(x, T, C, ldx, n_doy, n_years, spec, o, st);
-      if (e == 1) e = launch_day_lists(need, window, x, T, C, ldx, n_doy, n_years, spec, o, st);
-    } else {
-      e = upload_tables();  // a uniform calendar without a fast instantiation still needs the table
-      if (e) return e;
-      // Days whose samples decompose into per-day lists: the window must stay inside the year
-      // ([h, L_int - h)) and no window centre may fall outside the series (the h days before the first
-      // step's day-of-year and after the last step's: their neighbours exist but their centres do not).
-      std::vector<char> fast_day((size_t)n_doy, 0);
-      if (fast_ok) {
-        for (int d = h; d < L_int - h; ++d) fast_day[d] = 1;
-        const int s0 = doy_index_host[0] - 1, e1 = doy_index_host[T - 1] - 1;
-        for (int d = s0 - h; d < s0; ++d)
-          if (d >= 0) fast_day[d] = 0;
-        for (int d = e1 + 1; d <= e1 + h; ++d)
-          if (d < n_doy) fast_day[d] = 0;
-      }
-      for (int a = 0; a < n_doy;) {
-        int b = a;
-        const bool fast = fast_day[a] != 0;
-        while (b < n_doy && (fast_day[b] != 0) == fast) ++b;
-        if (fast && (b - a) >= 8)
-          e = launch_day_lists(need, window, x, T, C, ldx, n_doy, n_years, spec, o, st, posrow_d, n_doy, a, b);
-        else
-          e = launch_generic(need, x, T, C, ldx, pos_d, n_doy, n_years, h, spec, o, st, a, b, vrow_d);
-        if (e) return e;
-        a = b;
-      }
-    }
+  for (const PdoyLaunch& ln : plan.launches) {
+    const int32_t e = launch_pdoy(ln, x, T, C, ldx, n_doy, n_years, window, pos_d, posrow_d, vrow_d,
+                                  out + (int64_t)ln.ip * n_doy * C, sms, st);
     if (e) return e;
   }
   return XC_OK;
@@ -1225,7 +1092,11 @@ extern "C" int32_t xc_percentile_doy_generic_f32(const float* x, int64_t T, int6
     set_error("percentile needs %d order statistics; at most 64 are kept", need);
     return XC_ERR_UNSUPPORTED;
   }
-  return launch_generic(need, x, T, C, ldx, (const int32_t*)workspace, n_doy, n_years, window / 2, spec, out, st);
+  const int sms = sm_count();
+  PdoyLaunch ln = pdoy_generic(need, 0, 0, n_doy, C, sms);
+  ln.spec = spec;
+  return launch_pdoy(ln, x, T, C, ldx, n_doy, n_years, window, (const int32_t*)workspace, nullptr, nullptr, out, sms,
+                     st);
 }
 
 extern "C" int32_t xc_doy_interp_f64(const double* table, int32_t n_src, int64_t C, int32_t doy_min,

@@ -23,12 +23,11 @@
 #include <algorithm>
 #include <type_traits>
 
+#include "launch_plan.cuh"
 #include "runstat.cuh"
 
 namespace xc {
 namespace {
-
-constexpr int kThreads = 128;
 
 // ------------------------------------------------------------------------------------------------
 // threshold count (+ valid count)
@@ -629,15 +628,9 @@ period_multi_kernel(const float* __restrict__ x, int64_t C, int64_t ldx, const i
 template <int NC, int NCR, int NM, int NS>
 int32_t launch_multi(const float* x, int64_t C, int64_t ldx, const int32_t* poff, int32_t P, const XcMultiPlan& plan,
                      float* out, cudaStream_t st) {
-  // 4 cells per thread only pays for the lightest passes (measured: conditional sums are bound by the
-  // float32 -> float64 conversions on the XU pipe, more conditions by registers)
-  if constexpr (NCR == 0 && NM == 0 && NS == 0 && NC <= 2) {
-    period_multi_kernel<NC, NCR, NM, NS, 4, 8><<<grid_for(C, 4, P), kThreads, 0, st>>>(x, C, ldx, poff, plan, out,
-                                                                                        (int64_t)P * C);
-  } else {
-    period_multi_kernel<NC, NCR, NM, NS, 2, 12><<<grid_for(C, 2, P), kThreads, 0, st>>>(x, C, ldx, poff, plan, out,
-                                                                                         (int64_t)P * C);
-  }
+  constexpr MultiShape s = multi_shape(NC, 2 * NCR, NM, NS);
+  period_multi_kernel<NC, NCR, NM, NS, s.vec, s.unroll><<<grid_for(C, s.vec, P), kThreads, 0, st>>>(
+      x, C, ldx, poff, plan, out, (int64_t)P * C);
   return launch_status("period_multi_kernel");
 }
 
@@ -845,40 +838,12 @@ extern "C" int32_t xc_period_multi_f32(const float* x, int64_t T, int64_t C, int
   XC_REQUIRE(T < (1LL << 24), "xc_period_multi_f32 counts in float32: time axis must be shorter than 2^24 steps, got %lld",
              (long long)T);
   XcMultiPlan pl = *plan_host;
-  XC_REQUIRE(pl.n_cond >= 0 && pl.n_cond <= XC_MULTI_MAX_COND && pl.n_runs >= 0 && pl.n_runs <= XC_MULTI_MAX_RUNS &&
-                 pl.n_runs % 2 == 0 && pl.n_msum >= 0 && pl.n_msum <= XC_MULTI_MAX_MSUM && pl.n_sums >= 0 &&
-                 pl.n_sums <= XC_MULTI_MAX_SUMS,
-             "plan holds at most %d conditions, %d run outputs (an even number), %d run sums and %d conditional sums",
-             XC_MULTI_MAX_COND, XC_MULTI_MAX_RUNS, XC_MULTI_MAX_MSUM, XC_MULTI_MAX_SUMS);
-  XC_REQUIRE(pl.n_runs / 2 <= pl.n_cond && (pl.n_msum == 0 || pl.n_cond > 0), "run outputs need their condition");
   XC_REQUIRE(can_vec4(x, C, ldx, out, nullptr), "xc_period_multi_f32 needs C, ldx multiples of 4 and 16-byte aligned buffers");
-  auto slot_ok = [&](int32_t sl) { return sl >= -1 && sl < n_slots; };
-  bool ok = slot_ok(pl.slot_sum) && slot_ok(pl.slot_mean) && slot_ok(pl.slot_min) && slot_ok(pl.slot_max);
-  // entries beyond the declared counts are neutralised (the rounded-up instantiation computes and drops them)
-  for (int j = 0; j < XC_MULTI_MAX_COND; ++j) {
-    if (j >= pl.n_cond) { pl.cond[j].slot_n = pl.cond[j].slot_max = -1; pl.cond[j].wmax = 1; pl.cond[j].sgn = 0.f; pl.cond[j].thr = 0.f; }
-    ok = ok && slot_ok(pl.cond[j].slot_n) && slot_ok(pl.cond[j].slot_max);
-  }
-  for (int k = 0; k < XC_MULTI_MAX_RUNS; ++k) {
-    if (k >= pl.n_runs) { pl.runs[k].slot = -1; pl.runs[k].cond = k / 2; pl.runs[k].window = 1; pl.runs[k].kind = 0; }
-    ok = ok && slot_ok(pl.runs[k].slot) && pl.runs[k].window >= 1 && (pl.runs[k].kind == 0 || pl.runs[k].kind == 1) &&
-         pl.runs[k].cond == k / 2;
-  }
-  for (int k = 0; k < XC_MULTI_MAX_MSUM; ++k) {
-    if (k >= pl.n_msum) { pl.msum[k].slot = -1; pl.msum[k].cond = 0; pl.msum[k].window = 1; }
-    ok = ok && slot_ok(pl.msum[k].slot) && pl.msum[k].window >= 1 && pl.msum[k].cond == 0;
-  }
-  for (int k = 0; k < XC_MULTI_MAX_SUMS; ++k) {
-    if (k >= pl.n_sums) { pl.sums[k].slot = -1; pl.sums[k].mode = 0; }
-    ok = ok && slot_ok(pl.sums[k].slot) && (pl.sums[k].mode == 0 || pl.sums[k].mode == 1);
-  }
-  XC_REQUIRE(ok, "plan: output slot outside [-1, n_slots), window < 1 or run output not at its condition's place");
+  if (int32_t ep = check_multi_plan(pl, n_slots)) return ep;
   cudaStream_t st = (cudaStream_t)stream;
   float* o = (float*)out;
-  const int ncr = pl.n_runs / 2;
-  int nc = pl.n_cond == 0 ? 0 : (pl.n_cond <= 2 ? 2 : (pl.n_cond <= 4 ? 4 : 6));
-  const int nm = pl.n_msum;
-  const int ns = pl.n_sums == 0 ? 0 : 3;
+  const MultiShape sh = multi_shape(pl.n_cond, pl.n_runs, pl.n_msum, pl.n_sums);
+  const int nc = sh.nc, ncr = sh.ncr, nm = sh.nm, ns = sh.ns;
 #define XC_MULTI(CN, R, M, S) \
   if (nc == CN && ncr == R && nm == M && ns == S) return launch_multi<CN, R, M, S>(x, C, ldx, period_offsets, P, pl, o, st)
 #define XC_MULTI_C(CN)                                                                                   \

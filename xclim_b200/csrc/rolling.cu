@@ -11,6 +11,7 @@
 // window are re-read from L1/L2 (the rows were just fetched by the same warp), so DRAM traffic stays
 // one read of the input.  These are the low-volume members of the family (the window == 1 fast
 // kernels in period_stats.cu carry the headline configurations); operators are runtime switches.
+#include "launch_plan.cuh"
 #include "runstat.cuh"
 #include <limits>
 #include <type_traits>
@@ -18,8 +19,6 @@
 
 namespace xc {
 namespace {
-
-constexpr int kThreads = 128;
 
 // A switch on the uniform operator, not bivariate.cu's branch-free OpMask: with the mask form the
 // compute-bound spell_runstat4_kernel runs about 14% slower.
@@ -175,8 +174,7 @@ struct BlockStream {
     i = start;
     primed = false;
   }
-  // short windows are cheaper to re-read (L1 hits) than to slide with float64 adds
-  __device__ __forceinline__ bool sliding() const { return (wstat == XC_STAT_SUM || wstat == XC_STAT_MEAN) && w > 6; }
+  __device__ __forceinline__ bool sliding() const { return block_stream_slides(wstat, w); }
   // qualifies(block starting at i) ; advances to i + 1.  Caller guarantees i + w <= T.
   __device__ __forceinline__ bool next() {
     float r;
@@ -755,11 +753,12 @@ inline SumRange make_sum_range(int op, float thr, int w, bool mean) {
   return g;
 }
 
+// spell_sumw_kernel<W, RED, AFTER> with the plan's RED (the run-length reducer stays a run-time argument)
 template <int W, bool AFTER>
-int32_t launch_spell_sumw_red(const float* x, int64_t T, int64_t C, int64_t ldx, const int32_t* poff, int32_t P,
-                              const SumRange& g, int32_t reducer, float* out, cudaStream_t st) {
+int32_t launch_spell_sumw(const float* x, int64_t T, int64_t C, int64_t ldx, const int32_t* poff, int32_t P,
+                          const SumRange& g, int32_t red, int32_t reducer, float* out, cudaStream_t st) {
   dim3 grid((unsigned)((C / 4 + kThreads - 1) / kThreads), (unsigned)P, 1);
-  switch (reducer) {
+  switch (red) {
     case XC_RL_MAX: spell_sumw_kernel<W, XC_RL_MAX, AFTER><<<grid, kThreads, 0, st>>>(x, T, C, ldx, poff, g, reducer, out); break;
     case XC_RL_SUM: spell_sumw_kernel<W, XC_RL_SUM, AFTER><<<grid, kThreads, 0, st>>>(x, T, C, ldx, poff, g, reducer, out); break;
     case XC_RL_COUNT: spell_sumw_kernel<W, XC_RL_COUNT, AFTER><<<grid, kThreads, 0, st>>>(x, T, C, ldx, poff, g, reducer, out); break;
@@ -768,41 +767,29 @@ int32_t launch_spell_sumw_red(const float* x, int64_t T, int64_t C, int64_t ldx,
   return launch_status("spell_sumw_kernel");
 }
 
-template <int W>
-int32_t launch_spell_sumw(const float* x, int64_t T, int64_t C, int64_t ldx, const int32_t* poff, int32_t P,
-                          const SumRange& g, int32_t reducer, bool after, float* out, cudaStream_t st) {
-  return after ? launch_spell_sumw_red<W, true>(x, T, C, ldx, poff, P, g, reducer, out, st)
-               : launch_spell_sumw_red<W, false>(x, T, C, ldx, poff, P, g, reducer, out, st);
-}
-
+// rolling_sumw_kernel<W, MODE> with the plan's MODE
 template <int W>
 int32_t launch_rolling_sumw(const float* x, int64_t T, int64_t C, int64_t ldx, const int32_t* poff, int32_t P,
-                            int32_t is_mean, int32_t shift, int32_t stat, float* out, cudaStream_t st) {
+                            int32_t mode, int32_t is_mean, int32_t shift, int32_t stat, float* out, cudaStream_t st) {
   dim3 grid((unsigned)((C / 4 + kThreads - 1) / kThreads), (unsigned)P, 1);
-  if (stat == XC_STAT_MAX)
+  if (mode == 0)
     rolling_sumw_kernel<W, 0><<<grid, kThreads, 0, st>>>(x, T, C, ldx, poff, is_mean, shift, stat, out);
-  else if (stat == XC_STAT_MIN)
+  else if (mode == 1)
     rolling_sumw_kernel<W, 1><<<grid, kThreads, 0, st>>>(x, T, C, ldx, poff, is_mean, shift, stat, out);
   else
     rolling_sumw_kernel<W, 2><<<grid, kThreads, 0, st>>>(x, T, C, ldx, poff, is_mean, shift, stat, out);
   return launch_status("rolling_sumw_kernel");
 }
 
-#define XC_DISPATCH_W(w, CALL)          \
-  switch (w) {                          \
-    case 2: return CALL(2);             \
-    case 3: return CALL(3);             \
-    case 4: return CALL(4);             \
-    case 5: return CALL(5);             \
-    case 6: return CALL(6);             \
-    case 7: return CALL(7);             \
-    case 8: return CALL(8);             \
-    default: break;                     \
+// f(W) for the window w of a register-kernel plan, W in [kRegisterWMin, kRegisterWMax]
+template <int W = kRegisterWMin, typename F>
+int32_t dispatch_register_window(int w, F&& f) {
+  if constexpr (W > kRegisterWMax) {
+    set_error("no register kernel for window %d", w);
+    return XC_ERR_INVALID;
+  } else {
+    return w == W ? f(std::integral_constant<int, W>{}) : dispatch_register_window<W + 1>(w, f);
   }
-
-// the streaming kernels need 16-byte aligned rows and a ring that fits shared memory
-inline bool can_stream4(const float* x, int64_t C, int64_t ldx, const float* out, int32_t w) {
-  return (C % 4 == 0) && (ldx % 4 == 0) && aligned16(x) && aligned16(out) && (size_t)w * kThreads * 16 <= 160 * 1024;
 }
 
 
@@ -921,17 +908,16 @@ extern "C" int32_t xc_rolling_period_reduce_f32(const float* x, int64_t T, int64
                  window_stat == XC_STAT_MAX,
              "window statistic must be sum, mean, min or max");
   XC_REQUIRE(stat >= XC_STAT_SUM && stat <= XC_STAT_COUNT, "unknown reduction %d", stat);
-  if (center && window % 2 == 0) {
-    set_error("centred rolling windows of even length are not supported");
-    return XC_ERR_UNSUPPORTED;
-  }
-  if (can_stream4(x, C, ldx, out, window) && (window_stat == XC_STAT_SUM || window_stat == XC_STAT_MEAN)) {
+  RollPlan pl;
+  if (int32_t e = plan_rolling(C, ldx, aligned16(x), aligned16(out), window, window_stat, center, stat, &pl)) return e;
+  if (pl.family == kRollingSumw) {
     const int32_t is_mean = (window_stat == XC_STAT_MEAN) ? 1 : 0, shift = center ? window / 2 : 0;
-#define XC_CALL_ROLL(W) launch_rolling_sumw<W>(x, T, C, ldx, period_offsets, P, is_mean, shift, stat, out, (cudaStream_t)stream)
-    XC_DISPATCH_W(window, XC_CALL_ROLL)
-#undef XC_CALL_ROLL
+    return dispatch_register_window(pl.window, [&](auto WC) {
+      return launch_rolling_sumw<decltype(WC)::value>(x, T, C, ldx, period_offsets, P, pl.arg, is_mean, shift, stat,
+                                                      out, (cudaStream_t)stream);
+    });
   }
-  if (can_stream4(x, C, ldx, out, window)) {
+  if (pl.family == kRollingReduce4) {
     const size_t smem = (size_t)window * kThreads * 16;
     if (smem > 48 * 1024)
       XC_CHECK_CUDA(cudaFuncSetAttribute(rolling_period_reduce4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -975,13 +961,19 @@ extern "C" int32_t xc_spell_runstat_f32(const float* x, int64_t T, int64_t C, in
              "window reducer must be sum, mean, min or max");
   XC_REQUIRE(op >= XC_OP_GT && op <= XC_OP_NE, "Operation `%d` not recognized.", op);
   XC_REQUIRE(reducer >= XC_RL_MAX && reducer <= XC_RL_STD, "unknown run-length reducer %d", reducer);
-  if (can_stream4(x, C, ldx, out, window) && (window_stat == XC_STAT_SUM || window_stat == XC_STAT_MEAN)) {
+  const RollPlan pl = plan_spell(C, ldx, aligned16(x), aligned16(out), window, window_stat, reducer,
+                                 resample_before_rl == 0);
+  if (pl.family == kSpellSumw) {
     const SumRange g = make_sum_range(op, (float)thr, window, window_stat == XC_STAT_MEAN);
-#define XC_CALL_SPELL(W) launch_spell_sumw<W>(x, T, C, ldx, period_offsets, P, g, reducer, resample_before_rl == 0, out, (cudaStream_t)stream)
-    XC_DISPATCH_W(window, XC_CALL_SPELL)
-#undef XC_CALL_SPELL
+    return dispatch_register_window(pl.window, [&](auto WC) {
+      constexpr int W = decltype(WC)::value;
+      return pl.after ? launch_spell_sumw<W, true>(x, T, C, ldx, period_offsets, P, g, pl.arg, reducer, out,
+                                                   (cudaStream_t)stream)
+                      : launch_spell_sumw<W, false>(x, T, C, ldx, period_offsets, P, g, pl.arg, reducer, out,
+                                                    (cudaStream_t)stream);
+    });
   }
-  if (can_stream4(x, C, ldx, out, window)) {
+  if (pl.family == kSpellRunstat4) {
     const size_t smem = (size_t)window * kThreads * 16;
     dim3 grid4((unsigned)((C / 4 + kThreads - 1) / kThreads), (unsigned)P, 1);
     auto go = [&](auto AFTC) -> int32_t {
@@ -991,12 +983,12 @@ extern "C" int32_t xc_spell_runstat_f32(const float* x, int64_t T, int64_t C, in
                                                               (float)thr, reducer, out);
       return launch_status("spell_runstat4_kernel");
     };
-    return resample_before_rl ? go(std::false_type{}) : go(std::true_type{});
+    return !pl.after ? go(std::false_type{}) : go(std::true_type{});
   }
   dim3 grid((unsigned)((C + kThreads - 1) / kThreads), (unsigned)P, 1);
   spell_runstat_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(x, T, C, ldx, period_offsets, window,
                                                                     window_stat, op, (float)thr, reducer,
-                                                                    resample_before_rl ? 0 : 1, out);
+                                                                    pl.after ? 1 : 0, out);
   return launch_status("spell_runstat_kernel");
 }
 
